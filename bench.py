@@ -1,13 +1,13 @@
 #!/usr/bin/env python3
-"""bench.py - candidate plans evaluated / second on B200 (BASELINE.json metric).
+"""bench.py - candidate plans evaluated / second on H100 (BASELINE.json metric).
 
 A "step" is one full search of the workload's candidate space (every inter-stage plan enumerated by
 InterStagePlanGenerator, its intra-stage chain, load balancer and cost model) by libmetis_b200.so.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl reference] [--dump-outputs DIR]
 
 Workload: BASELINE.json configs[2] ("homo 64-GPU cluster, 96-layer GPT-3, gbs=512 (~10^6 candidates)
-- 1xB200, HBM-roofline capture"), i.e. c3_homo64_mpl6 = 771 750 inter-stage plans, the configuration the
+- 1xH100, HBM-roofline capture"), i.e. c3_homo64_mpl6 = 771 750 inter-stage plans, the configuration the
 metric is quoted on for one GPU; configs[1] (16 GPUs, 1 752 plans) is a parity-test case
 (tests/test_gpu_parity.py).  N > 1 shards the same space by plan ordinal over the ranks (strong scaling)
 with one NCCL all_gather of 32-byte best records per step.
@@ -28,10 +28,17 @@ Timed regions
           of the same plans, one process per usable host core: the unmodified reference from baseline/_ref when
           that directory exists (kind "reference"), else the oracle (Python port of the pure-Python reference,
           oracle/metis_oracle.py, kind "port").
+  Both GPU regions run exactly K timed steps.
+
+--dump-outputs DIR: after the timed steps, what the last `value` step computed (rank 0's shard) as a caller of the
+search receives it: every costed candidate's record in estimate_costs order, one float64 .npy per field, and the
+summary (counters, best); a seeded sample of the records when they exceed 60 MB (the dump stays under 64 MB).  The inputs are generated from
+fixed seeds, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
 import statistics
@@ -247,11 +254,11 @@ def workload_config(name, num_plans):
 # GPU side
 # ---------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """Streams `nvidia-smi -lms 50` for one GPU while the timed regions run (B200_PROFILING.md clocks line)."""
+    """Streams `nvidia-smi -lms 50` for one GPU while the timed regions run (clocks, power limit, throttle reasons)."""
 
     QUERY = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
              'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
-             'clocks_event_reasons.sw_power_cap')
+             'clocks_event_reasons.sw_power_cap,power.limit')
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -265,6 +272,7 @@ class ClockSampler(threading.Thread):
             self.proc = subprocess.Popen(['nvidia-smi', f'--id={self.index}', f'--query-gpu={self.QUERY}',
                                           '--format=csv,noheader,nounits', '-lms', '50'],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.stop)          # a run that raises must not leave nvidia-smi streaming
             for line in self.proc.stdout:
                 if self.armed.is_set() and line.strip():
                     self.rows.append([x.strip() for x in line.strip().split(',')])
@@ -273,19 +281,47 @@ class ClockSampler(threading.Thread):
 
     def stop(self):
         self.armed.clear()
-        if self.proc is not None:
+        if self.proc is not None and self.proc.poll() is None:
             self.proc.terminate()
+            self.proc.wait()
 
     def summary(self):
         if not self.rows:
-            return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['nvidia-smi unavailable']}
+            return {'sm_mhz': None, 'sm_max_mhz': None, 'power_limit_w': None, 'reasons': ['nvidia-smi unavailable']}
         sm = [float(r[0]) for r in self.rows if r[0].replace('.', '').isdigit()]
         mx = [float(r[1]) for r in self.rows if r[1].replace('.', '').isdigit()]
+        pl = [float(r[7]) for r in self.rows if len(r) > 7 and r[7].replace('.', '').isdigit()]
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
         reasons = [n for i, n in enumerate(names) if any(r[3 + i].lower().startswith('active') for r in self.rows)]
         return {'sm_mhz': statistics.median(sm) if sm else None, 'sm_max_mhz': max(mx) if mx else None,
-                'reasons': reasons, 'samples': len(self.rows),
+                'power_limit_w': max(pl) if pl else None, 'reasons': reasons, 'samples': len(self.rows),
                 'window': 'device-timed steps + end-to-end steps (both keep the GPU busy)'}
+
+
+DUMP_BYTES = 60 * 10 ** 6          # records; the whole dump stays under 64 MB
+
+
+def dump_outputs(out_dir, searcher, stream):
+    """--dump-outputs: the records of the searcher's last launch in estimate_costs order (the device sort
+    HetSearcher.run applies), one float64 array per field, plus the summary; records beyond DUMP_BYTES are
+    thinned to a fixed, seeded sample (kept in order)."""
+    from metis_b200 import native
+    sm = searcher.summary()
+    n = int(sm.num_records)
+    searcher.sort_records(n, native.SORT_POSITION, stream)
+    stream.synchronize()
+    rec = searcher.records[:2 * n].cpu().numpy().view(native.RECORD_DTYPE)
+    fields = [f for f, _ in native.RECORD_DTYPE]
+    keep = DUMP_BYTES // (8 * len(fields))
+    if n > keep:
+        rec = rec[np.sort(np.random.default_rng(0).choice(n, keep, replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    for f in fields:
+        np.save(os.path.join(out_dir, f'records_{f}.npy'), rec[f].astype(np.float64))
+    b = sm.best
+    summary = [sm.num_records, sm.num_partition_calls, sm.num_balancer_runs, sm.num_keyerror,
+               b.cost, b.ordinal, b.step, b.num_repartition, b.num_stage]
+    np.save(os.path.join(out_dir, 'summary.npy'), np.array(summary, dtype=np.float64))
 
 
 def run_ours(ns, emit=True):
@@ -402,9 +438,11 @@ def run_ours(ns, emit=True):
         dist.all_reduce(kmean, op=dist.ReduceOp.MAX)
     ms_per_step = float(total_ms.item()) / ns.steps
     kernel_ms = float(kmean.item())
+    if ns.dump_outputs and rank == 0:
+        dump_outputs(ns.dump_outputs, full, stream)
 
     # ---- e2e: the drop-in API call from host inputs, every step -----------------------------------
-    e2e_steps = max(3, min(ns.steps, 10))
+    e2e_steps = ns.steps
     e2e_wall, parts = [], []
     res = None
     for i in range(e2e_steps + 2):                            # two warm-up calls: engine creation, buffer growth
@@ -441,12 +479,8 @@ def run_ours(ns, emit=True):
             peaks = json.load(open(os.path.join(REPO, 'MEASURED_PEAKS.json')))
         except Exception:
             pass
-        peak = float(peaks.get('hbm_gbs', 6650.0))
+        peak = float(peaks.get('hbm_gbs', 3350.0))
         achieved = alg_bytes / world / (kernel_ms * 1e-3) / 1e9
-        traffic = None                                        # measured for the 1-GPU launch only
-        tpath = os.path.join(REPO, 'profiles', 'r02_traffic.json')
-        if os.path.exists(tpath) and world == 1:
-            traffic = json.load(open(tpath)).get('dram_bytes_per_search')
         eng = api._ENGINES.get((local, rank, world))
         h2d = int(eng[0].h2d_bytes) if eng else int(dp.h2d_bytes)
         n_rec = counters['num_records'] if world > 1 else len(ref.records)
@@ -482,12 +516,14 @@ def run_ours(ns, emit=True):
                           'note': 'search_kernels = het_admit + het_scatter + het_first + het_chain (CUDA events '
                                   'recorded by the library around those four launches)'},
             'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
-                         'frac': achieved / peak, 'traffic': traffic,
-                         'peak_source': 'MEASURED_PEAKS.json hbm_gbs (measured)' if 'hbm_gbs' in peaks else 'fallback',
+                         'frac': achieved / peak,
+                         'peak_source': 'MEASURED_PEAKS.json hbm_gbs (measured)' if 'hbm_gbs' in peaks else
+                                        'H100 SXM data sheet (3.35 TB/s HBM3), not measured',
                          'algorithmic_bytes_per_launch': alg_bytes // world,
                          'note': 'S+16 B read per inter-stage plan + 16 B written per costed candidate (SURVEY.md 8d) over '
                                  'the time of the four search kernels (the chain kernel dominates); the path is '
                                  'fp64-latency / instruction-issue bound, not HBM bound'},
+            'gpu': torch.cuda.get_device_name(dev),
             'clocks': sampler.summary() if sampler else None,
             'wall_s_timed_region': wall,
         }
@@ -518,7 +554,10 @@ def main():
     ap.add_argument('--cpu-sample', type=int, default=3000, help='plans per host core for cpu_baseline')
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--no-extra', action='store_true', help='skip the configs[3] measurements reported under `extra`')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the last timed step\'s results as DIR/<name>.npy')
     ns = ap.parse_args()
+    if ns.steps < 1:
+        ap.error('--steps must be at least 1')
     # stdout carries exactly one JSON line: libraries that write to fd 1 (NCCL prints its version there when
     # NCCL_DEBUG=VERSION) are sent to stderr for the duration of the run
     global _RESULT_FD
@@ -528,7 +567,7 @@ def main():
     if ns.impl == 'reference':
         run_reference_arm(ns)
         return
-    # --workload a,b,c (developer use: the scaling table of profiles/) runs the workloads one after the other in
+    # --workload a,b,c (developer use: scaling tables) runs the workloads one after the other in
     # this process group and prints one line each; the default invocation prints exactly one line
     names = ns.workload.split(',')
     if names == [DEFAULT_WORKLOAD] and not ns.no_extra:
@@ -538,7 +577,7 @@ def main():
         extra = {}
         for name in EXTRA_WORKLOADS:
             sub = argparse.Namespace(**vars(ns))
-            sub.workload, sub.steps, sub.no_cpu = name, min(ns.steps, 5), True
+            sub.workload, sub.no_cpu, sub.dump_outputs = name, True, None
             try:
                 other = run_ours(sub, emit=False)
             except Exception as exc:                          # noqa: BLE001 - the headline line must still be printed

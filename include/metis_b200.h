@@ -1,5 +1,5 @@
 /*
- * metis_b200.h - C ABI of libmetis_b200.so (hand-written sm_100a CUDA).
+ * metis_b200.h - C ABI of libmetis_b200.so (hand-written sm_90a CUDA).
  *
  * The reference (SamsungLabs/Metis @ ed41176) is pure Python and has no FFI
  * layer; its seam for the plan-search hot path is the pair of Python functions

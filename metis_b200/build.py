@@ -1,4 +1,4 @@
-"""In-tree build of libmetis_b200.so (nvcc, sm_100a only) and of the oracle's C pieces."""
+"""In-tree build of libmetis_b200.so (nvcc, sm_90a only)."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ LIB = os.path.join(HERE, 'libmetis_b200.so')
 SOURCES = ['metis_search.cu', 'metis_rank.cu', 'metis_enum.cpp']
 HEADERS = ['metis_eval.cuh', 'metis_coop.cuh', 'metis_trace.cuh', 'metis_rows.cuh', 'metis_internal.h', os.path.join('..', '..', 'include', 'metis_b200.h')]
 
-NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo',
+NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
               '-fmad=false',            # parity: no FMA contraction (CPython evaluates a*b+c in two roundings)
               '-diag-suppress', '128,20168',   # unreachable loop in one instantiation; '#pragma unroll 0' = compiler default
               '-Xcompiler', '-fPIC', '-shared']

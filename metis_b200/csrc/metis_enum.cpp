@@ -240,7 +240,7 @@ class WorkerPool {
   private:
     WorkerPool() : pid_(getpid()) {
         const char *env = getenv("METIS_ENUM_THREADS");
-        unsigned v = env ? (unsigned)atoi(env) : 8u;         // 8 host threads measured best on the B200 hosts
+        unsigned v = env ? (unsigned)atoi(env) : 8u;         // 8 host threads unless METIS_ENUM_THREADS says otherwise
         const unsigned hw = std::thread::hardware_concurrency();
         if (hw && v > hw) v = hw;
         if (v < 1) v = 1;

@@ -238,7 +238,7 @@ MB_HD double py_sum_range(const double *x, int a, int b) {
 }
 
 // The same, kept out of line and rolled: the cooperative mode is instruction-fetch bound
-// (profiles/: stall_no_instruction is its top stall), so it trades unrolling for code size.
+// (stall_no_instruction is its top stall), so it trades unrolling for code size.
 MB_HD_NOINLINE double py_sum_range_compact(const double *x, int a, int b) {
     if (a >= b) return 0.0;
     double f = 0.0 + x[a];

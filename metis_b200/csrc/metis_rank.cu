@@ -171,7 +171,7 @@ using namespace metis;
 
 extern "C" {
 
-// upper bound on the warps of the cooperative grid (B200: 148 SMs x 2 blocks x 8 warps)
+// upper bound on the warps of the cooperative grid (H100 SXM: 132 SMs x 2 blocks x 8 warps = 2112)
 static const int64_t kRankMaxWarps = 8192;
 
 int64_t metis_sort_workspace_bytes(int64_t n) {

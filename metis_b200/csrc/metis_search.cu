@@ -1,4 +1,4 @@
-// metis_search.cu - sm_100a kernels + C ABI of libmetis_b200.so (see include/metis_b200.h).
+// metis_search.cu - sm_90a kernels + C ABI of libmetis_b200.so (see include/metis_b200.h).
 //
 // Kernel map (SURVEY.md section 8a):
 //   het_rows_kernel       a3/a4: device-group rows of every composition, in the reference's visiting order
@@ -23,7 +23,7 @@
 //   layer_balance_kernel  a10 alone, for unit parity
 //   (rank_records_kernel, the stable record sort, lives in metis_rank.cu)
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false (no FMA contraction: parity).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (no FMA contraction: parity).
 #include <cuda_runtime.h>
 #include <cooperative_groups.h>
 #include <stdint.h>
@@ -40,16 +40,16 @@ namespace cg = cooperative_groups;
 
 namespace metis {
 
-// block shape measured on B200 (profiles/): 256 threads, >= 3 blocks/SM (80 registers) beat 128 x 6 and 256 x 4
+// bulk-round block shape: 256 threads, >= 3 blocks/SM, i.e. at most 80 registers (3 x 256 x 80 fits the 64 Ki
+// registers of an H100 SM); the other choices were 128 x 6 and 256 x 4
 #ifndef METIS_THREADS
 #define METIS_THREADS 256
 #endif
 #ifndef METIS_MIN_BLOCKS
 #define METIS_MIN_BLOCKS 3
 #endif
-// instantiations for more than 64 stages: 80 registers cost 80 B of spills and buy a third block per SM (measured:
-// BASELINE configs[3] 149 -> 140 ms); single-type clusters gain from a fourth one at 64 registers (128 GPUs / 1 type /
-// mpl 6: 24.6 -> 20.9 -> 19.5 ms), mixed-type ones lose (configs[3] at mpl 4: 9.96 -> 10.2 ms)
+// instantiations for more than 64 stages: 80 registers cost some spills and buy a third block per SM; single-type
+// clusters take a fourth one at 64 registers (more spills, more warps), mixed-type ones keep three
 #ifndef METIS_MIN_BLOCKS_BIG
 #define METIS_MIN_BLOCKS_BIG METIS_MIN_BLOCKS
 #endif

@@ -1,6 +1,6 @@
 """ctypes binding of libmetis_b200.so (C ABI declared in include/metis_b200.h).
 
-The library is built in-tree by ``metis_b200.build.build_library`` (nvcc, sm_100a).
+The library is built in-tree by ``metis_b200.build.build_library`` (nvcc, sm_90a).
 There is no CPU fallback: if the shared object is missing or a call fails, an
 exception is raised.
 """
@@ -98,7 +98,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     if not os.path.exists(path):
         raise MetisNativeError(
             f'{path} is missing: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-            f'(nvcc, sm_100a). metis_b200 has no CPU fallback.')
+            f'(nvcc, sm_90a). metis_b200 has no CPU fallback.')
     lib = C.CDLL(path)
     lib.metis_last_error.restype = C.c_char_p
     lib.metis_abi_version.restype = C.c_int

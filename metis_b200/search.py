@@ -1,8 +1,8 @@
-"""Device-side plan search: the B200 replacement of the loops in cost_het_cluster.py:21-50
+"""Device-side plan search: the GPU replacement of the loops in cost_het_cluster.py:21-50
 and cost_homo_cluster.py:21-37 of the reference.
 
 PyTorch is used only for device buffers, streams and (multi-GPU) torch.distributed; all
-search arithmetic runs in libmetis_b200.so (hand-written sm_100a CUDA) behind the C ABI of
+search arithmetic runs in libmetis_b200.so (hand-written sm_90a CUDA) behind the C ABI of
 include/metis_b200.h.  There is no CPU path: without CUDA these functions raise.
 """
 from __future__ import annotations

@@ -2,15 +2,15 @@
 
 This module is a plain-Python restatement of the reference algorithm
 (SamsungLabs/Metis @ ed41176).  It exists so the CUDA path can be checked
-against something that runs anywhere (the GPU box has no /root/reference).
+against something that runs anywhere (the GPU machines have no checkout of the reference).
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
 ``--impl reference`` legs may import it.  The product package (metis_b200/)
 must never import it and has no CPU fallback.
 
 Parity pin: the reference ships no tests or golden vectors for this path
 (SURVEY.md section 4), so the oracle is pinned against outputs of the
-*unmodified reference executed in the build container*
-(tests/golden/make_golden.py imports /root/reference and dumps
+*unmodified reference*
+(tests/golden/make_golden.py imports a checkout of it and dumps
 tests/golden/*.json.gz; tests/test_oracle_vs_golden.py replays them).
 
 All float arithmetic is IEEE binary64 in the order the reference evaluates it.

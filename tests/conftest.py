@@ -13,7 +13,7 @@ if REPO not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on an H100 with -m gpu)')
     config.addinivalue_line('markers', 'slow: long-running CPU test')
 
 

@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
-"""Generate tests/golden/*.npz by executing the UNMODIFIED reference (/root/reference).
+"""Generate tests/golden/*.npz by executing the UNMODIFIED reference (SamsungLabs/Metis @ ed41176).
 
-Run in the build container only (the GPU box has no /root/reference):
+Run where a checkout of the reference exists (METIS_REFERENCE points at it); the tests only read the outputs:
 
-    PYTHONHASHSEED=0 python tests/golden/make_golden.py [name ...] [--procs 8]
+    METIS_REFERENCE=<checkout> PYTHONHASHSEED=0 python tests/golden/make_golden.py [name ...] [--procs 8]
 
 What is reference code and what is harness:
   * every arithmetic / enumeration step is the reference's own classes
@@ -40,7 +40,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
-REF = '/root/reference'
+REF = os.environ.get('METIS_REFERENCE', '')
 sys.path.insert(0, REPO)
 
 from metis_b200.workloads import WORKLOADS, Workload, materialize, profile_file_order  # noqa: E402
@@ -60,7 +60,7 @@ def import_reference():
     if _REF_CACHE is not None:
         return _REF_CACHE
     sys.path.insert(0, REF)
-    import utils as ref_utils                                   # /root/reference/utils.py
+    import utils as ref_utils                                   # <reference>/utils.py
 
     class DeviceType(Enum):
         A100 = "a100"
@@ -364,7 +364,7 @@ def golden_transcript(name: str):
     import gzip
     ref = import_reference()
     sys.path.insert(0, REF)
-    import cost_het_cluster as ref_main                         # /root/reference/cost_het_cluster.py
+    import cost_het_cluster as ref_main                         # <reference>/cost_het_cluster.py
     with tempfile.TemporaryDirectory() as root:
         if name == 'c1':
             fix = os.path.join(HERE, 'fixtures', 'c1')

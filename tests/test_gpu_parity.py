@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box).  Everything goes through the C ABI of
+"""GPU parity tests (run with -m gpu on an H100).  Everything goes through the C ABI of
 libmetis_b200.so via ctypes (metis_b200.native / metis_b200.search) and is compared bit-for-bit
 with (a) golden files produced by the unmodified reference and (b) the CPU oracle on the same
 seeded inputs.  Integer outputs (partitions, strategies, ordinals, counters) and fp64 costs must be

@@ -1,7 +1,7 @@
 """Pin the CPU oracle (oracle/metis_oracle.py) to outputs of the unmodified reference.
 
 The golden files were produced by tests/golden/make_golden.py, which imports
-/root/reference in the build container.  Everything here is exact: candidate
+a checkout of the reference.  Everything here is exact: candidate
 order, partitions, strategies and the bits of every fp64 cost.
 """
 import gzip

@@ -1,5 +1,5 @@
 import time, sys, os
-sys.path.insert(0,'/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from metis_b200 import flatten, native
 lib=native.load_library()
 best=1e9
