@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libmetis_b200.so')
 SOURCES = ['metis_search.cu', 'metis_rank.cu', 'metis_enum.cpp']
-HEADERS = ['metis_eval.cuh', 'metis_coop.cuh', 'metis_trace.cuh', 'metis_rows.cuh', 'metis_internal.h', os.path.join('..', '..', 'include', 'metis_b200.h')]
+HEADERS = ['metis_eval.cuh', 'metis_coop.cuh', 'metis_warp.cuh', 'metis_trace.cuh', 'metis_rows.cuh', 'metis_internal.h', os.path.join('..', '..', 'include', 'metis_b200.h')]
 
 NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
               '-fmad=false',            # parity: no FMA contraction (CPython evaluates a*b+c in two roundings)

@@ -28,10 +28,6 @@
 
 #include "metis_eval.cuh"
 
-#ifdef METIS_HOST_STATS
-extern "C" void metis_host_stats(int slot, long add);
-#endif
-
 namespace metis {
 
 // Scalars a SEQ section hands to the following sections (per-warp scratch next to Scratch<>).
@@ -80,6 +76,7 @@ struct OneLane {
     MB_HD int incl_scan(int v) const { return v; }
     MB_HD int last_lane(int v) const { return v; }
     MB_HD void mark(int) const {}
+    MB_HD void note(int) const {}
     MB_HD void gate() const {}
 };
 
@@ -445,7 +442,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     MB_HD bool forward_coop() {
         const int S = pd.S, last = S - 1;
         const int L = T.p.num_layers;
-        if (S < 4 || T.p.norm_len < L) return false;          // nothing to overlap: sequential pass
+        if (S < 4 || T.p.norm_len < L) { x.note(kPathSeqForward); return false; }   // nothing to overlap: sequential pass
         const int N = kH * L;
         const int lim = (N - 1 - kH) > 0 ? (N - 1 - kH) : 0;  // :218
         const double *dsub = T.dsub;
@@ -462,7 +459,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                 int i0 = a + span - 14;                       // a 32-entry window around the expected end
                 if (i0 < a + 1) i0 = a + 1;
                 int i = x.first_ge_window(P, N, i0, a + 1, t);
-                if (i < 0) i = x.first_ge(P, N, t);
+                if (i < 0) { x.note(kPathFirstGe); i = x.first_ge(P, N, t); }
                 b = i - 1 > a ? i - 1 : a;
                 if (b >= lim) b = lim; else closed = true;
                 span = b - a;
@@ -488,11 +485,8 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
             if ((e & kBroke) && !bad && c > dsub[b]) bad = true;      // the reference would have gone on
             w.capa[s] = c;
         }
-#ifdef METIS_HOST_STATS
-        metis_host_stats(2, 1);
-        if (bad) metis_host_stats(15, 1);
-#endif
         if (x.any(bad)) {
+            x.note(kPathVerifyFailed);
             x.sync();
             METIS_PAR(x, s, last) w.capa[s] = w.perf[s];      // restore the input of the sequential pass
             return false;
@@ -516,7 +510,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     //               leader, general sequential form.
     //   middle      the block [k, m) between forward and backward fills, ascending: arg-max over [lo, last] by the
     //               whole warp per sub-layer.
-    // Writes w.capa, w.fe, w.lstk, w.blk, mail.k / m.  returns METIS_FATAL_* (0 = ok)
+    // Writes w.capa, w.fe, w.lstk, the middle block's stages (bytes of w.subw), mail.k / m.  returns METIS_FATAL_* (0 = ok)
     MB_HD int fill_coop() {
         const int S = pd.S, last = S - 1;
         const double *dlay = T.dlay;
@@ -536,6 +530,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         x.mark(12);
         const FillState st{mail.k, mail.s_top, mail.top_skip != 0};
         const int m = mail.m;
+        if (st.s_top >= 0 && !st.top_skip) x.note(kPathTail);
         // ---- skipped sub-layers ----
         // stages 0 .. reach hold the forward intervals; regular = none of them is empty
         const int reach = st.s_top;                           // -1 when S == 1
@@ -546,6 +541,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         }
         irregular = x.any(irregular);
         if (irregular) {
+            x.note(kPathIrregular);
             if (x.leader()) mail.err = seq_skipped<MAXS, MAXL>(T, S, w);
             x.sync();
             if (mail.err) return mail.err;
@@ -595,9 +591,9 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
             }
             x.sync();
         }
-        // ---- middle block ----
-        if (m - st.k > Scratch<MAXS, MAXL>::kBlock) return METIS_FATAL_SCRATCH;
+        // ---- middle block: any length up to 7 * L, one byte per sub-layer in w.subw (unused by the balancer else) ----
         if (m > st.k) {
+            x.note(kPathMiddle);
             if (x.leader()) mail.flag = middle_lo<MAXS, MAXL>(S, w, st);
             x.sync();
             int lo = mail.flag;
@@ -612,7 +608,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                 x.sync();                                     // every lane has read the capacities
                 if (x.leader()) {
                     w.capa[pick] = best - dlay[j / kH];
-                    w.blk[j - st.k] = (uint8_t)pick;
+                    reinterpret_cast<uint8_t *>(w.subw)[j - st.k] = (uint8_t)pick;
                 }
                 x.sync();
                 if (pick != last) lo = pick;                  // the nearest block item below that is not on `last`
@@ -638,7 +634,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         x.mark(13);
         // ---- majority vote back to real layers (:290-308), one layer per lane ----
         // Stage of sub-layer j, from the interval ends: j >= m -> last stage (backward tail); k <= j < m -> where
-        // the middle block put it (blk); below k the forward slot t = #{u : start of stage u+1 <= j}, and if j is
+        // the middle block put it (bytes of subw); below k the forward slot t = #{u : start of stage u+1 <= j}, and if j is
         // that slot's skipped sub-layer: last stage when the backward pass took it, else where it was placed (lstk).
         const int kfwd = mail.k;
         METIS_PAR(x, r, L) {
@@ -666,7 +662,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                     const int j = j0 + q;
                     int st;
                     if (j >= m) st = last;
-                    else if (j >= kfwd) st = w.blk[j - kfwd];
+                    else if (j >= kfwd) st = reinterpret_cast<const uint8_t *>(w.subw)[j - kfwd];
                     else {
 #pragma unroll 1
                         while (nxt <= j) { ++t; e = w.fe[t]; nxt = (int)(e & kPos) + ((e & kBroke) ? 1 : 0); }

@@ -154,6 +154,18 @@ MB_HD uint64_t pack_geo(int64_t row_offset, int S, int label, int ns, int div) {
            ((uint64_t)(ns & 0xFF) << 48) | ((uint64_t)(div & 0xFF) << 56);
 }
 
+// Paths of the layer balancer that the inputs decide (balance_run below, CoopEvaluator::balance_coop in
+// metis_coop.cuh).  The balancer tells its lane policy which ones a run takes (x.note); the policies of the product
+// ignore it, the test-only device build (tests/devsim) records it so that a test can show that its inputs reach them.
+enum BalancerPath {
+    kPathVerifyFailed = 0,   // coop: a predicted forward interval did not verify, the leader re-ran the forward pass
+    kPathSeqForward = 1,     // coop: fewer than 4 stages, the forward pass ran sequentially without a prediction
+    kPathIrregular = 2,      // a stage's forward interval is empty (coop: the leader places the skipped sub-layers)
+    kPathMiddle = 3,         // sub-layers are left between the forward and backward passes (the middle block)
+    kPathFirstGe = 4,        // coop: a prediction missed its 32-entry window and searched the whole table
+    kPathTail = 5,           // the forward pass ran into the reserved last 8 sub-layers with stages to spare
+};
+
 // Execution policies.  `Serial`: one thread owns the task (host, replay kernel, and the throughput
 // mode of the search kernel where the 32 lanes of a warp hold 32 different tasks).  A cooperative
 // policy (metis_search.cu: WarpLanes) has all lanes of a warp work on ONE task whose scratch lives in
@@ -169,6 +181,7 @@ struct Serial {
     MB_HD double max_all(double v) const { return v; }
     MB_HD bool any(bool p) const { return p; }
     MB_HD void mark(int) const {}              // profiling hook (cooperative mode, profiling build)
+    MB_HD void note(int) const {}              // balancer path taken (BalancerPath; recorded by tests/devsim only)
     // lockstep hooks (see Lockstep below): nothing to do when a thread works alone
     MB_HD void converge() const {}
     MB_HD void rejoin(bool) {}
@@ -201,7 +214,6 @@ constexpr uint16_t kPos = 0x3FFF;
 // allows, so that the per-thread arrays are accessed coalesced across the warp).
 template <int MAXS, int MAXL>
 struct Scratch {
-    static constexpr int kBlock = MAXS + 64;   // leftover sub-layers between the forward and backward fills
     double perf[MAXS];     // stage compute performance of the current attempt (sc_capa_bak)
     double capa[MAXS];     // working capacities / scratch
     double mstate[MAXS];   // memory_state of the last partition_layer call / scratch in adjust
@@ -214,9 +226,9 @@ struct Scratch {
     uint8_t tpc[MAXS];     // log2(tp)
     uint8_t lstk[MAXS];    // stage on which the skipped sub-layer of stage s was placed
     uint8_t got[MAXS];     // stage received a leftover sub-layer
-    uint8_t blk[kBlock];   // stage of each leftover of the middle block
     uint64_t ownerw[MAXL / 8 + 1];   // byte r = stage owning real layer r after the vote (kDropped = none)
-    uint64_t subw[MAXL];   // per real layer: byte q = stage of sub-layer 7r+q (below the backward tail)
+    uint64_t subw[MAXL];   // per real layer: byte q = stage of sub-layer 7r+q (below the backward tail); the chain
+                           // evaluator keeps the stages of the middle block here instead (byte j - k, up to 7 * MAXL)
 };
 
 // ---------------------------------------------------------------------------
@@ -516,6 +528,7 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
             if (s_in < last) w.subw[r] = v;
         }
         if (s < last) {                                          // ran into the reserved tail
+            x.note(kPathTail);
             w.capa[s] = c;
             w.fe[s] = (uint16_t)lim;
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -577,6 +590,7 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
             if (pos > start) {
                 lo = s;                                       // common case: stage s itself ends right below j
             } else {
+                x.note(kPathIrregular);
 #pragma unroll (X::kUniform ? 1 : 0)
                 for (int u = s;; --u) {
                     if (u < s) {                              // skipped sub-layer of stage u (already placed)
@@ -608,8 +622,8 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
         }
     }
     x.converge();
-    int nblk = m - k;
-    if (nblk > Scratch<MAXS, MAXL>::kBlock) { broken = METIS_FATAL_SCRATCH; nblk = Scratch<MAXS, MAXL>::kBlock; }
+    const int nblk = m - k;                                   // any length up to 7 * L: the picks go to subw
+    if (nblk > 0) x.note(kPathMiddle);
     {
         int below = -1;                                       // stage of the nearest block item not on `last`
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -637,7 +651,6 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
             for (int t2 = lo + 1; t2 <= last; ++t2)
                 if (w.capa[t2] > best) { best = w.capa[t2]; pick = t2; }
             w.capa[pick] -= dlay[j / kH];
-            w.blk[t] = (uint8_t)pick;
             if (pick != last) below = pick;
             sub_store(w.subw, j, pick);
         }

@@ -130,6 +130,18 @@ struct HostSink {
     }
 };
 
+// the host policies with a record of the balancer paths taken (bit p of *notes = BalancerPath p, metis_eval.cuh)
+struct NoteSerial : Serial {
+    unsigned *notes;
+    void note(int p) const { *notes |= 1u << p; }
+};
+struct NoteLane : OneLane {
+    unsigned *notes;
+    void note(int p) const { *notes |= 1u << p; }
+};
+// found by argument-dependent lookup ahead of the generic template: keeps OneLane's reverse order of PAR iterations
+int par_index(const NoteLane &x, int i, int n) { return x.reverse ? n - 1 - i : i; }
+
 }  // namespace
 
 extern "C" {
@@ -291,6 +303,58 @@ int hostsim_layer_balance(const double *capa, const int32_t *num_stage, int64_t 
         const int rc = balance_run<kS, kL>(T, S, w, Serial());
         if (rc) { out[0] = 0xFFFF; continue; }
         for (int s = 0; s <= S; ++s) out[s] = w.part[s];
+    }
+    return 0;
+}
+
+// One balancer form over n rows, like tests/devsim's devsim_balance: policy 0 = balance_run (Serial), 1 = balance_coop
+// (OneLane), 2 = balance_coop visiting the PAR iterations in reverse.  The tables are derived from a minimal problem
+// (no keys, batch sizes or tp) by derive_entry, so the predictor of the forward pass sees the bits a search gives it.
+// Per row: partition, METIS_FATAL_* code, BalancerPath bits and the middle block's length (coop; -1 for Serial).
+int hostsim_balance(int32_t policy, const double *capa, const int32_t *num_stage, int64_t n, int32_t stride,
+                    const double *lc, int32_t norm_len, int32_t num_layers, uint16_t *partition, int32_t *rc,
+                    uint32_t *notes, int32_t *block) {
+    if (policy < 0 || policy > 2 || num_layers > kL) return -1;
+    for (int64_t i = 0; i < n; ++i)
+        if (num_stage[i] < 1 || num_stage[i] > kS || num_stage[i] > stride) return -1;
+    MetisProblem p;
+    memset(&p, 0, sizeof(p));
+    p.num_layers = num_layers;
+    p.norm_len = norm_len;
+    const double bw[1] = {1.0};
+    const DerivedLayout d = derived_layout(p);
+    std::vector<double> derived(d.total + 1);
+    for (int i = 0; i < d.total; ++i) derived[i] = derive_entry(p, d, lc, nullptr, bw, i);
+    Tables T;
+    memset(&T, 0, sizeof(T));
+    T.p = p;
+    T.norm_lc = lc;
+    bind_derived(T, derived.data());
+    static thread_local Scratch<kS, kL> w;
+    static thread_local CoopMail mail;
+    for (int64_t i = 0; i < n; ++i) {
+        const int S = num_stage[i];
+        for (int s = 0; s < S; ++s) w.perf[s] = capa[i * stride + s];
+        unsigned got = 0;
+        int r, blk = -1;
+        if (policy == 0) {
+            NoteSerial x;
+            x.notes = &got;
+            r = balance_run<kS, kL>(T, S, w, x);
+        } else {
+            NoteLane x;
+            x.notes = &got;
+            x.reverse = policy == 2;
+            CoopEvaluator<kS, kL, NoteLane> ev(T, w, mail, x);
+            ev.pd.S = S;
+            r = ev.balance_coop();
+            if (!r) blk = mail.m > mail.k ? mail.m - mail.k : 0;
+        }
+        rc[i] = r;
+        notes[i] = got;
+        block[i] = blk;
+        if (!r)
+            for (int s = 0; s <= S; ++s) partition[i * (stride + 1) + s] = w.part[s];
     }
     return 0;
 }
