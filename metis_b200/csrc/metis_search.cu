@@ -207,6 +207,17 @@ __device__ __forceinline__ void stage_blob_tma(uint8_t *smem, const uint8_t *blo
     }
 }
 
+// Tables of a search kernel: one descriptor per block, in shared memory, written by thread 0 while the tables are
+// staged.  A copy per thread (the whole MetisProblem and the table pointers, ~430 B) would live in local memory,
+// and every read of a launch constant (T.p.num_layers, T.rsum, ...) would be a local load.  Called by all threads.
+__device__ __forceinline__ const Tables &block_tables(Tables &s_tables, const MetisProblem &p, const BlobLayout &lay,
+                                                      const uint8_t *blob, uint8_t *smem, int use_smem, uint64_t *mbar) {
+    if (threadIdx.x == 0) s_tables = make_tables(p, lay, use_smem ? smem : blob, blob);
+    if (use_smem) stage_blob_tma(smem, blob, lay.total, mbar);     // its __syncthreads publishes s_tables
+    else __syncthreads();
+    return s_tables;
+}
+
 // ---- ordinal -> plan ---------------------------------------------------------------------------
 __device__ __forceinline__ int find_block(const MetisPlanSpace &sp, int64_t ordinal) {
     int lo = 0, hi = sp.num_blocks - 1;
@@ -471,15 +482,11 @@ het_first_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
                  const __grid_constant__ DeviceOut out, const SearchLists ls, const int best_slot) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
+    __shared__ Tables s_tables;
     DeviceSink sink(out);
     const unsigned int n = ls.ctl[0];
     if ((long long)n >= ls.bulk_min) {
-        const uint8_t *base = blob;
-        if (use_smem) {
-            stage_blob_tma(smem, blob, lay.total, &mbar);
-            base = smem;
-        }
-        const Tables T = make_tables(p, lay, base, blob);
+        const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
         Scratch<MAXS, MAXL> w;
         const int lane = threadIdx.x & 31;
         for (;;) {                                           // batches of 32 plans, longest stage counts first
@@ -555,12 +562,8 @@ het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
                  const int best_slot) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
-    const uint8_t *base = blob;
-    if (use_smem) {
-        stage_blob_tma(smem, blob, lay.total, &mbar);
-        base = smem;
-    }
-    const Tables T = make_tables(p, lay, base, blob);
+    __shared__ Tables s_tables;
+    const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
     DeviceSink sink(out);
     const int lane = threadIdx.x & 31;
     sink.leader = lane == 0;
@@ -906,10 +909,9 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
             const unsigned int off = chain_smem_tables ? blob_pad : 0u;
             const size_t dyn = off + (size_t)(threads / 32) * per_warp;
             if (dyn > (size_t)smem_optin) continue;
-            if (dyn > 48 * 1024) {
-                e = cudaFuncSetAttribute(chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-                if (e != cudaSuccess) { cudaGetLastError(); continue; }
-            }
+            // always set: the default limit is 48 KB minus the kernel's static shared memory, not 48 KB
+            e = cudaFuncSetAttribute(chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+            if (e != cudaSuccess) { cudaGetLastError(); continue; }
             int per_sm = 0;
             e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chain, threads, dyn);
             if (e != cudaSuccess || per_sm < 1) { cudaGetLastError(); continue; }
@@ -919,20 +921,16 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
         if (chain_threads == 0) chain_smem_tables = 0;
     }
     if (chain_threads == 0) return arg_fail("chain kernel does not fit this device (shared memory)");
-    if (chain_dyn > 48 * 1024) {
-        e = cudaFuncSetAttribute(chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chain_dyn);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(chain)");
-    }
+    e = cudaFuncSetAttribute(chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chain_dyn);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(chain)");
     int64_t chain_grid = (int64_t)sms * chain_per_sm;
 
     // ---- bulk round ----
     auto first = het_first_kernel<MAXS, MAXL, ONE>;
     int first_smem_tables = (int)lay.total <= blob_max && blob_pad <= (unsigned int)smem_optin;
     size_t first_dyn = first_smem_tables ? blob_pad : 0;
-    if (first_dyn > 48 * 1024) {
-        e = cudaFuncSetAttribute(first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_dyn);
-        if (e != cudaSuccess) { cudaGetLastError(); first_smem_tables = 0; first_dyn = 0; }
-    }
+    e = cudaFuncSetAttribute(first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_dyn);
+    if (e != cudaSuccess) { cudaGetLastError(); first_smem_tables = 0; first_dyn = 0; }   // static + blob too large
     int first_per_sm = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&first_per_sm, first, kThreads, first_dyn);
     if (e != cudaSuccess || first_per_sm < 1) return cuda_fail(e, "occupancy query (bulk round)");
