@@ -9,6 +9,7 @@ from typing import List
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libmetis_b200.so')
+PROF_LIB = os.path.join(HERE, 'libmetis_b200_prof.so')
 SOURCES = ['metis_search.cu', 'metis_rank.cu', 'metis_enum.cpp']
 HEADERS = ['metis_eval.cuh', 'metis_coop.cuh', 'metis_warp.cuh', 'metis_trace.cuh', 'metis_rows.cuh', 'metis_internal.h', os.path.join('..', '..', 'include', 'metis_b200.h')]
 
@@ -25,22 +26,25 @@ def nvcc_path() -> str:
     raise RuntimeError('nvcc not found: cannot build libmetis_b200.so')
 
 
-def stale() -> bool:
-    if not os.path.exists(LIB):
+def stale(lib: str = LIB) -> bool:
+    if not os.path.exists(lib):
         return True
-    t = os.path.getmtime(LIB)
+    t = os.path.getmtime(lib)
     deps: List[str] = [os.path.join(CSRC, s) for s in SOURCES + HEADERS]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_library(force: bool = False, verbose: bool = False) -> str:
-    if not force and not stale():
-        return LIB
-    cmd = [nvcc_path()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + \
-          ['-o', LIB] + [os.path.join(CSRC, s) for s in SOURCES]
+def build_library(force: bool = False, verbose: bool = False, profile: bool = False) -> str:
+    """profile=True builds PROF_LIB instead: the same library with the chain kernel's phase clock
+    (-DMETIS_PROFILE_PHASES, read by tools/phase_profile.py).  Never loaded by a search."""
+    lib = PROF_LIB if profile else LIB
+    if not force and not stale(lib):
+        return lib
+    cmd = [nvcc_path()] + NVCC_FLAGS + (['-DMETIS_PROFILE_PHASES'] if profile else []) + \
+          (['-Xptxas', '-v'] if verbose else []) + ['-o', lib] + [os.path.join(CSRC, s) for s in SOURCES]
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if proc.returncode != 0:
         raise RuntimeError(f'nvcc failed:\n{proc.stdout}\n{proc.stderr}')
     if verbose:
         print(proc.stderr)
-    return LIB
+    return lib

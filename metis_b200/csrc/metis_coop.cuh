@@ -77,8 +77,12 @@ struct OneLane {
     MB_HD int last_lane(int v) const { return v; }
     MB_HD void mark(int) const {}
     MB_HD void note(int) const {}
-    MB_HD void gate() const {}
+    MB_HD void gate(int, int) const {}
 };
+
+// Block gates of a balancer run (ChainCoop::gate), in the order a run reaches them
+enum CoopGate { kGateRun = 0, kGateBackward = 1, kGateLeftover = 2, kGateVote = 3, kGateAdjust = 4, kGateMemory = 5,
+                kGateCost = 6 };
 
 // index of PAR iteration number `i` (0-based count of this lane's iterations) - lets the host policy reverse
 template <class X>
@@ -517,17 +521,19 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         x.sync();
         const bool fwd = forward_coop();
         x.sync();
+        x.gate(kGateBackward, 11);
         if (x.leader()) {
             if (!fwd) {
+                x.mark(18);
                 const FillState st = seq_forward<MAXS, MAXL>(T, S, w);
                 mail.k = st.k; mail.s_top = st.s_top; mail.top_skip = st.top_skip ? 1 : 0;
+                x.mark(11);
             }
-            x.mark(11);
             mail.m = seq_backward<MAXS, MAXL>(T, S, w, mail.k);
             mail.err = 0;
         }
         x.sync();
-        x.mark(12);
+        x.gate(kGateLeftover, 12);
         const FillState st{mail.k, mail.s_top, mail.top_skip != 0};
         const int m = mail.m;
         if (st.s_top >= 0 && !st.top_skip) x.note(kPathTail);
@@ -592,6 +598,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
             x.sync();
         }
         // ---- middle block: any length up to 7 * L, one byte per sub-layer in w.subw (unused by the balancer else) ----
+        x.mark(17);
         if (m > st.k) {
             x.note(kPathMiddle);
             if (x.leader()) mail.flag = middle_lo<MAXS, MAXL>(S, w, st);
@@ -631,7 +638,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         const int rc_tail = fill_coop();
         if (rc_tail) return rc_tail;
         const int m = mail.m;
-        x.mark(13);
+        x.gate(kGateVote, 13);
         // ---- majority vote back to real layers (:290-308), one layer per lane ----
         // Stage of sub-layer j, from the interval ends: j >= m -> last stage (backward tail); k <= j < m -> where
         // the middle block put it (bytes of subw); below k the forward slot t = #{u : start of stage u+1 <= j}, and if j is
@@ -700,7 +707,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
             w.capa[s] = n ? w.perf[s] - range_sum<SerialUniform>(T, kRangeNorm, 0, lc, w.first[s], (int)w.lastl[s] + 1) : w.perf[s];
         }
         x.sync();
-        x.mark(15);
+        x.gate(kGateAdjust, 15);
         // ---- boundary adjustment (:310-356): at most three committed single-layer moves ----
         uint8_t *owner = reinterpret_cast<uint8_t *>(w.ownerw);
 #pragma unroll 1
@@ -1018,10 +1025,10 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                 for (int a = first_attempt; a <= 3; ++a) {    // LayerLoadBalancer.partition_layer (:121-144)
                     if (!skip_first) sink.balancer_run();
                     skip_first = false;
-                    x.gate();                                 // (device) the block's warps start their runs together
+                    x.gate(kGateRun, 9);                      // gate points (ChainCoop::gate): the block meets at the vote
                     rc = balance_coop();
                     if (rc) { sink.fatal(pd.ordinal, rc, aux); return; }
-                    x.mark(20);
+                    x.gate(kGateMemory, 20);
                     const int r = memory_phase_coop(a);
                     if (r < 0) { sink.fatal(pd.ordinal, -r, aux); return; }
                     if (r == 1) { attempt = a; break; }
@@ -1032,7 +1039,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                 if (attempt > 0) break;
             }
             nrep = attempt;
-            x.mark(22);
+            x.gate(kGateCost, 22);
             double cost = 0.0;
             if (get_cost_coop(cost) == 0) sink.emit(pd, step, nrep, cost, w.tpc, w.part);
             else sink.keyerror();

@@ -563,6 +563,7 @@ het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
     __shared__ Tables s_tables;
+    WarpCoop::prof_init();                                   // (phase clock build only; published by block_tables)
     const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
     DeviceSink sink(out);
     const int lane = threadIdx.x & 31;
@@ -572,8 +573,8 @@ het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
     const bool bulk = (long long)n_adm >= ls.bulk_min;
     const uint4 *list = ls.b;                                // sorted: by chain hint after a bulk round, else by stage count
     const unsigned int n = bulk ? ls.ctl[2] : n_adm;
-    WarpCoop lanes;
-    CoopEvaluator<MAXS, MAXL, WarpCoop, ONE> ev(T, cs->w, cs->mail, lanes);
+    ChainCoop lanes;
+    CoopEvaluator<MAXS, MAXL, ChainCoop, ONE> ev(T, cs->w, cs->mail, lanes);
     for (;;) {
         unsigned int i = 0;
         if (lane == 0) i = atomicAdd(&ls.ctl[3], 1u);
@@ -582,15 +583,17 @@ het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
         const uint4 e = __ldcg(&list[i]);
         PlanDesc pd;
         decode_entry(sp, e, pd);
-        lanes.mark(1);
+        ev.x.mark(1);                                        // the evaluator's own clock: one phase at a time
         // flags: not touched by a bulk round -> kFresh; else what first_task decided (kReplay / kRetry / kAdvance)
         const int start = (e.y & 1u) ? (int)((e.y >> 1) & 3u) : 0;
         const double *perf = nullptr;
         if (start == 2) perf = ls.perf + __ldcg(&ls.src[i]);
         ev.run_chain(pd, sink, start, perf, (size_t)ls.save_cap);
-        lanes.mark(0);
+        ev.x.mark(0);
     }
+    ev.x.mark(25);
     while (WarpCoop::block_or(0)) {}                         // out of work: answer the others' gates until all are done
+    ev.x.mark(31);
     sink.leader = true;                                      // lanes 1-31 carry empty counters / bests
     if (lane != 0) { sink.n_part = sink.n_run = sink.n_key = 0; }
     finish_block(sink, out, best_slot + blockIdx.x);
