@@ -19,10 +19,12 @@
 // Control flow outside SEQ sections is uniform (every lane takes the same branches because the conditions are
 // reduction results or values read from the scratch after a sync).
 //
-// The per-stage helpers of PlanEvaluator (metis_eval.cuh: mixed-type stages, bandwidth selection, memory
-// capacity) are reused unchanged: inside a PAR section the lane that owns the stage calls them on its own copy
-// of the evaluator.  Plain C++ (the policy supplies the warp primitives) so that tests/hostsim can compile the
-// same source with g++; the host policy has one lane and can visit the PAR iterations in reverse order, which
+// The cost model of one stage (PlanEvaluator::stage_performance, stage_memory, stage_adjust, stage_time and
+// stage_terms in metis_eval.cuh) is shared with the one-plan-per-thread evaluator: inside a PAR section the lane
+// that owns the stage calls it on its own copy of the evaluator and stores the results to the warp's scratch.  What
+// differs by design stays here: the reductions, the order-dependent sums (leader lane) and which scratch the results
+// go to.  Plain C++ (the policy supplies the warp primitives) so that tests/hostsim can compile the same source with
+// g++; the host policy has one lane and can visit the PAR iterations in reverse order, which
 // catches a dependence between iterations without a GPU.
 #pragma once
 
@@ -35,7 +37,7 @@ struct CoopMail {
     int m;        // first sub-layer of the backward tail (LayerComputeBalancer state)
     int err;      // METIS_FATAL_* raised inside a SEQ section
     int flag;     // generic boolean result
-    int pad;
+    int aux;      // aux value of err
     double val;   // generic fp64 result (totals)
     double val2;
     int k;        // end of the forward pass: first sub-layer not offered to a forward stage
@@ -380,45 +382,27 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
 #pragma unroll 1
             for (int s = 0; s < n; ++s)
                 if (box[s] != 0.0) {
-                    const uint64_t code = (uint64_t)box[s];
-                    mail.err = (int)(code & 0xFF);
-                    mail.pad = (int)(code >> 8);
+                    uint32_t a;
+                    mail.err = decode_error(box[s], a);
+                    mail.aux = (int)a;
                     break;
                 }
         }
         x.sync();
-        aux = (uint32_t)mail.pad;
+        aux = (uint32_t)mail.aux;
         return mail.err;
     }
 
     // StagePerformance.get_intra_stage_compute_performance (model/device_group.py:54-85) -> w.perf
     MB_HD int compute_performance_coop() {
-        const bool one_type = ONE || T.p.num_types == 1;
         bool failed = false;
         x.sync();
         METIS_PAR(x, s, pd.S) {
-            const int g = w.gcode[s], tpc = w.tpc[s];
-            double p = 0.0;
-            int fail = 0;
-            int ta = 0, tb = 0;
-            if (!one_type) {
-                const int a = this->rank_start(s), b = a + (1 << g);
-                ta = type_of_rank(T, pd.ns, a); tb = type_of_rank(T, pd.ns, b - 1);
-            }
-            if (ta == tb) {
-                const int bs = bs_total >> (g - tpc);
-                const int key = key_of(T, ta, tpc, bs);
-                if (key < 0) { aux = ((uint32_t)tpc << 16) | (uint32_t)bs; fail = METIS_FATAL_KEY_EXEC; }
-                else if (T.exec_full[key] == 0.0) fail = METIS_FATAL_ZERODIV;
-                else p = T.inv_exec[key];                     // 1. / profile_cost
-            } else {
-                const int a = this->rank_start(s);
-                const int rc = this->hetero_performance(a, a + (1 << g), 1 << (g - tpc), tpc, p);
-                if (rc) fail = rc;
-            }
+            double p;
+            const int rc = this->stage_performance(s, p);
             w.perf[s] = p;
-            w.extra[s] = fail ? (double)fail + (double)aux * 256.0 : 0.0;   // per-stage error mailbox
-            failed = failed || fail != 0;
+            w.extra[s] = encode_error(rc, aux);
+            failed = failed || rc != 0;
         }
         if (x.any(failed)) return first_error(w.extra, pd.S);
         x.sync();
@@ -771,35 +755,20 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // in: w.perf (c_capa), w.extra (m_demand); out: w.perf; returns 1 = None, 0 ok, <0 fatal (negated code)
     MB_HD int adjust_performance_coop() {
         const int S = pd.S;
-        const bool one_type = ONE || T.p.num_types == 1;
         double *ratio = reinterpret_cast<double *>(w.subw);      // free after the vote (MAXL >= MAXS)
-        double *mcap = ratio + MAXS / 2;                          // stage memory capacity; subw has MAXL >= 2*(MAXS/2).. see static_assert
-        static_assert(MAXL >= MAXS, "subw doubles as two S-sized fp64 arrays only when MAXL >= 2 * MAXS / 2");
-        (void)mcap;
         x.sync();
         METIS_PAR(x, s, S) {                                     // independent per stage (:80-89)
-            const int a = one_type ? 0 : this->rank_start(s), b = a + this->group(s);
-            const double c = w.perf[s], md = w.extra[s];
-            const double mc = one_type ? T.type_memory[0] * (double)this->group(s) : this->memory_capacity(a, b);
-            double av, adj;
-            if (mc > md) {
-                adj = c;
-                av = (c * mc / md) - c;
-            } else {
-                av = 0.0;
-                adj = c * (mc / md) * 0.9;
-            }
+            double av, adj, extra;
+            this->stage_adjust(s, av, adj, extra);
             w.capa[s] = av;           // available_compute_capacity
             w.mstate[s] = adj;        // adj_sc_capa
-            ratio[s] = (mc > md) ? 0.0 : (c - adj);          // this stage's term of extra_required_capacity (:89)
+            ratio[s] = extra;         // this stage's term of extra_required_capacity
         }
         x.sync();
         if (x.leader()) {                                        // order-dependent accumulations (:89-91)
             double need = 0.;
 #pragma unroll 4
-            for (int s = 0; s < S; ++s)
-                if (w.capa[s] == 0.0 && ratio[s] != 0.0) need += ratio[s];
-                else if (ratio[s] != 0.0) need += ratio[s];
+            for (int s = 0; s < S; ++s) need += ratio[s];
             mail.val = need;
             mail.flag = seq_py_sum(w.capa, S) < need ? 1 : 0;
         }
@@ -843,35 +812,15 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // memory demand (:29-55), OOM test (:57-63), capacity re-weighting.  Returns like PlanEvaluator::memory_phase.
     MB_HD int memory_phase_coop(int attempt) {
         const int S = pd.S;
-        const bool one_type = ONE || T.p.num_types == 1;
-        const int type0 = T.run_type[pd.ns * T.p.num_types];
-        const bool q10_short = T.p.q10_devices < T.p.total_devices;   // node 0 has fewer GPUs than the average (Q10)
-        const bool own_type = (T.p.corrected & METIS_FIX_Q6) != 0;
         bool failed = false, oom = false;
         x.sync();                                            // the balancer's last readers of capa / extra / mstate are done
         METIS_PAR(x, s, S) {
-            const int g = w.gcode[s], tpc = w.tpc[s];
-            const int a = this->rank_start(s), b = a + (1 << g);
-            double md = 0.001, err = 0.0;
-            if (!ONE && own_type) {                          // opt-in METIS_FIX_Q6 (not the reference; single type: no change)
-                const int rc = this->memory_demand_own_type(s, md);
-                if (rc) err = (double)rc + (double)aux * 256.0;
-            } else if (q10_short && !own_type && b > T.p.q10_devices) {
-                err = (double)METIS_FATAL_INDEX;             // device_types[rank]: IndexError (load_balancer.py:36, Q10)
-            } else if (one_type || type_of_q10(T, pd.ns, a) == type_of_q10(T, pd.ns, b - 1)) {
-                const int bs = bs_total >> (g - tpc);
-                const int key = key_of(T, type0, tpc, bs);
-                if (key < 0) err = (double)METIS_FATAL_KEY_MEMORY + (double)(((uint32_t)tpc << 16) | (uint32_t)bs) * 256.0;
-                else md += range_sum<SerialUniform>(T, kRangeMem, key, T.mem + (size_t)key * T.p.lpad, w.part[s], w.part[s + 1]) * kMemCoef;
-            } else {
-                const int rc = this->hetero_memory_demand(s, type0, md);
-                if (rc) err = (double)rc + (double)aux * 256.0;
-            }
-            const double state = one_type ? T.type_memory[0] * (double)(1 << g) - md : this->memory_capacity(a, b) - md;
+            double md, state;
+            const int rc = this->stage_memory(s, md, state);
             w.extra[s] = md;
             w.capa[s] = state;
-            w.mstate[s] = err;
-            failed = failed || err != 0.0;
+            w.mstate[s] = encode_error(rc, aux);
+            failed = failed || rc != 0;
             oom = oom || state < 0;
         }
         failed = x.any(failed);
@@ -893,10 +842,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // HeteroCostEstimator.get_cost (model/cost_estimator.py:199-244); returns 0 ok, 1 KeyError.  The cost lands in
     // mail.val (every lane reads it after the final sync).
     MB_HD int get_cost_coop(double &cost_out) {
-        const int per = T.p.devices_per_node;
-        const int Lm = T.p.num_layers;
         const bool one_type = ONE || T.p.num_types == 1;
-        const bool ubw = T.p.uniform_bw != 0;
         const int nstage = pd.label < pd.S ? pd.label : pd.S;  // zip(range(plan.num_stage), strategies)
         // rank_node_map holds num_nodes * devices(node 0) ranks (cluster_bandwidth.py:34-47, Q10): beyond -> KeyError
         if (T.p.q10_devices < T.p.total_devices && this->rank_start(nstage) > T.p.q10_devices) return 1;
@@ -905,53 +851,12 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         double max_len = -INFINITY, max_upd = -INFINITY, max_dp = -INFINITY;
         x.sync();
         METIS_PAR(x, s, nstage) {
-            const int g = w.gcode[s], tpc = w.tpc[s];
-            const int a = one_type ? 0 : this->rank_start(s), b = a + (1 << g);
-            const int la = w.part[s], lb = w.part[s + 1];
-            const int ldp = g - tpc;
-            const int mbs = bs_total >> ldp;
-            const int ta = one_type ? 0 : type_of_rank(T, pd.ns, a);
-            const int tb = one_type ? 0 : type_of_rank(T, pd.ns, b - 1);
-            double len = 0.0;
-            if (ta == tb) {                                   // _get_execution_cost :175-188
-                const int key = key_of(T, ta, tpc, mbs);
-                if (key < 0) bad = true;
-                else len = range_sum<SerialUniform>(T, kRangeLc, key, T.lc + (size_t)key * T.p.lpad, la, lb);
-            } else if (this->hetero_exec_cost(a, b, 1 << ldp, tpc, la, lb, len)) {
-                bad = true;
-            }
+            double len, dpc, upd;
+            if (this->stage_time(s, len)) bad = true;
             w.capa[s] = len;
             if (len > max_len) max_len = len;
-            const double inv_tp = pow2_neg(tpc);              // 1 / tp, exact power of two
-            double pp = 0.0;
-            if (s < nstage - 1) {
-                if (ubw) {                                    // :224-227 via the derived tables
-                    pp = (lb == Lm - 1) ? T.pp_vocab[mbs * T.p.num_tp + tpc] : T.pp_hidden[mbs];
-                } else {
-                    double act;
-                    if (lb == Lm - 1)
-                        act = (double)((int64_t)mbs * T.p.sequence_length * T.p.vocab_size) * inv_tp;
-                    else
-                        act = (double)((int64_t)mbs * T.p.sequence_length * T.p.hidden_size);
-                    const int a2 = this->rank_start(s), b2 = this->rank_start(s + 2);
-                    pp = act / (this->bw_of_node_range(a2 / per, (b2 - 1) / per) * 1048576.0);
-                }
-            }
-            ppterm[s] = pp;
-            // get_parameter_size_by_stage (model/activation_parameter.py:40-51)
-            int ntr = lb - la;
-            double params = 0.0;
-            if (la == 0) { params += T.p.input_params * inv_tp; --ntr; }
-            if (lb == Lm) { params += T.p.output_params * inv_tp; --ntr; }
-            params += T.p.transformer_params * inv_tp * (double)ntr;
-            double dpc;                                       // :37-43
-            if (ubw) dpc = T.dpk[ldp] * params;
-            else {
-                const int dp = 1 << ldp;
-                dpc = (double)(2 * (dp - 1)) / ((double)dp * (this->dp_bandwidth(this->rank_start(s), dp, 1 << tpc) * 1048576.0)) * params;
-            }
+            this->stage_terms(s, nstage, ppterm[s], dpc, upd);
             if (dpc > max_dp) max_dp = dpc;
-            const double upd = T.p.optimizer_time * inv_tp * T.ratio[lb - la];   // :145-147
             if (upd > max_upd) max_upd = upd;
         }
         if (x.any(bad)) return 1;                             // KeyError raised while costing a stage

@@ -30,18 +30,6 @@
 
 namespace metis {
 
-// Task-list words are read with ld.global.cg (L2 only): in the barrier-free latency mode another SM may have
-// rewritten a neighbouring slot of the same 128-byte line a moment ago, and an L1 copy of that line fetched
-// by a different warp of this SM could be stale (L1 is not coherent; every task is read exactly once anyway).
-template <class V>
-MB_HD V list_load(const V *p) {
-#if defined(__CUDA_ARCH__)
-    return __ldcg(p);
-#else
-    return *p;
-#endif
-}
-
 constexpr int kH = 7;                 // hallucination (model/load_balancer.py:183)
 constexpr double kMemCoef = 5.0;      // mem_coef (model/load_balancer.py:31)
 constexpr uint8_t kDropped = 0xFF;    // real layer kept by no stage (quirk Q5)
@@ -166,21 +154,12 @@ enum BalancerPath {
     kPathTail = 5,           // the forward pass ran into the reserved last 8 sub-layers with stages to spare
 };
 
-// Execution policies.  `Serial`: one thread owns the task (host, replay kernel, and the throughput
-// mode of the search kernel where the 32 lanes of a warp hold 32 different tasks).  A cooperative
-// policy (metis_search.cu: WarpLanes) has all lanes of a warp work on ONE task whose scratch lives in
-// shared memory: loops over independent elements are strided over the lanes (lane()/width(), then
-// sync()), everything else is executed redundantly by every lane on identical data.
+// Policies of PlanEvaluator and balance_run, which always evaluate one plan in one thread.  `Serial`: the thread
+// works on its own (host build, replay and trace kernels, layer_balance_kernel).  `kUniform` picks rolled loops and
+// the out-of-line range sum where a policy cares more about code size than about unrolling.
 struct Serial {
     static constexpr bool kUniform = false;
-    MB_HD int lane() const { return 0; }
-    MB_HD int width() const { return 1; }
-    MB_HD void sync() const {}
-    // combine per-lane partial results: largest v, lowest index among equals / largest v
-    MB_HD void argmax_first(double &, int &) const {}
-    MB_HD double max_all(double v) const { return v; }
-    MB_HD bool any(bool p) const { return p; }
-    MB_HD void mark(int) const {}              // profiling hook (cooperative mode, profiling build)
+    MB_HD void mark(int) const {}              // profiling hook (chain kernel, profiling build)
     MB_HD void note(int) const {}              // balancer path taken (BalancerPath; recorded by tests/devsim only)
     // lockstep hooks (see Lockstep below): nothing to do when a thread works alone
     MB_HD void converge() const {}
@@ -200,7 +179,9 @@ struct Lockstep : Serial {
     __device__ void rejoin(bool p) { mask = __ballot_sync(0xFFFFFFFFu, p); }
 };
 #endif
-struct SerialUniform : Serial {           // tests: the code paths of the cooperative mode, one lane
+// `SerialUniform`: the base PlanEvaluator of the chain evaluator (metis_coop.cuh), whose per-stage members run in the
+// lane that owns the stage.  The chain kernel is bound by instruction fetch, so its code is kept small.
+struct SerialUniform : Serial {
     static constexpr bool kUniform = true;
 };
 
@@ -229,6 +210,7 @@ struct Scratch {
     uint64_t ownerw[MAXL / 8 + 1];   // byte r = stage owning real layer r after the vote (kDropped = none)
     uint64_t subw[MAXL];   // per real layer: byte q = stage of sub-layer 7r+q (below the backward tail); the chain
                            // evaluator keeps the stages of the middle block here instead (byte j - k, up to 7 * MAXL)
+    static_assert(MAXL >= MAXS, "after the vote, subw holds one double per stage (adjust_performance, get_cost)");
 };
 
 // ---------------------------------------------------------------------------
@@ -488,10 +470,8 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
                                                              // the end - an exit inside the loops below would keep
                                                              // the lanes of the bulk round from re-joining (Lockstep)
 
-    x.sync();                                                // lane-strided writes below: earlier readers are done
 #pragma unroll (X::kUniform ? 1 : 0)
-    for (int s = x.lane(); s < S; s += x.width()) { w.capa[s] = w.perf[s]; w.got[s] = 0; w.cnt[s] = 0; }
-    x.sync();
+    for (int s = 0; s < S; ++s) { w.capa[s] = w.perf[s]; w.got[s] = 0; w.cnt[s] = 0; }
 
     x.mark(10);
     // ---- forward pass (:216-231): flat scan, layer by layer, 7 sub-layers each -----------------
@@ -661,10 +641,9 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
     // ---- majority vote back to real layers (:290-308) ------------------------------------------
     // A stage holding >= 4 of a layer's 7 sub-layers holds the middle one or one of the first
     // three, so at most four candidates are counted (SWAR byte compare on the packed layer word).
-    x.sync();
     int run_own = (int)kDropped, run_first = 0, run_len = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
-    for (int r = x.lane(); r < L; r += x.width()) {
+    for (int r = 0; r < L; ++r) {
         const int nlow = m - kH * r;                         // sub-layers of r below the backward tail
         int own;
         if (nlow <= 0) {
@@ -697,15 +676,12 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
         w.lastl[run_own] = (uint16_t)(L - 1);
         w.cnt[run_own] = (uint16_t)(w.cnt[run_own] + run_len);
     }
-    x.sync();
     x.mark(14);
     x.converge();
     uint8_t *owner = reinterpret_cast<uint8_t *>(w.ownerw);
-    x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
-    for (int s = x.lane(); s < S; s += x.width())            // :300-306
+    for (int s = 0; s < S; ++s)                              // :300-306
         w.capa[s] = w.cnt[s] ? w.perf[s] - range_sum<X>(T, kRangeNorm, 0, lc, w.first[s], (int)w.lastl[s] + 1) : w.perf[s];
-    x.sync();
 
     x.mark(15);
     x.converge();
@@ -715,9 +691,8 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
         int top = 0x7FFFFFFF;
         double maxc = -INFINITY;
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int t = x.lane(); t < S; t += x.width())        // stable: lowest index among equal maxima (:329-331)
+        for (int t = 0; t < S; ++t)                          // stable: lowest index among equal maxima (:329-331)
             if (w.capa[t] > maxc) { maxc = w.capa[t]; top = t; }
-        x.argmax_first(maxc, top);
         if (top == 0x7FFFFFFF) top = 0;
         int nb = -1;
         double val = INFINITY;
@@ -730,13 +705,11 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
         const double nnb = w.capa[nb] + dl;
         double newmax = -INFINITY;
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int t = x.lane(); t < S; t += x.width()) {
+        for (int t = 0; t < S; ++t) {
             const double v = (t == top) ? ntop : (t == nb) ? nnb : w.capa[t];
             if (v > newmax) newmax = v;
         }
-        newmax = x.max_all(newmax);
         if (newmax > maxc) break;                            // :352 (not committed)
-        x.sync();
         owner[layer] = (uint8_t)top;
         w.capa[top] = ntop;
         w.capa[nb] = nnb;
@@ -749,7 +722,6 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
         }
         ++w.cnt[top];
         --w.cnt[nb];
-        x.sync();
     }
 
     x.mark(16);
@@ -857,6 +829,15 @@ MB_HD int halvings_of(const MetisProblem &p, int S, const uint8_t *gcode, const 
     return u;
 }
 
+// Per-stage error word: a stage's METIS_FATAL_* code and aux value in one double, 0.0 = no error.  A loop over the
+// stages stores one word per stage; the first nonzero word in stage order is the error the reference raises.
+MB_HD double encode_error(int rc, uint32_t aux) { return rc ? (double)rc + (double)aux * 256.0 : 0.0; }
+MB_HD int decode_error(double word, uint32_t &aux) {
+    const uint64_t code = (uint64_t)word;
+    aux = (uint32_t)(code >> 8);
+    return (int)(code & 0xFF);
+}
+
 template <int MAXS, int MAXL, class X = Serial, bool ONE = false>
 struct PlanEvaluator {
     const Tables &T;
@@ -897,7 +878,7 @@ struct PlanEvaluator {
         while ((2 << lb) <= bs_total) ++lb;
         nbad = 0;
         int a = 0;
-        for (int s = 0; s < pd.S; ++s) {                     // set_groups + first strategy in one pass
+        for (int s = 0; s < pd.S; ++s) {                     // groups, rank starts and first strategy in one pass
             const int g = pd.row[s];
             const int t = g > lb ? g - lb : 0;
             if (stage_bad(g, t)) { nbad = 1; return 0; }     // the plan can never become valid: drop it now
@@ -929,9 +910,7 @@ struct PlanEvaluator {
         if (pick < 0) return false;
         const int g = w.gcode[pick], t = w.tpc[pick];
         nbad += (stage_bad(g, t + 1) ? 1 : 0) - (stage_bad(g, t) ? 1 : 0);
-        x.sync();                                            // every lane has read tpc[pick] before any lane rewrites it
         w.tpc[pick] = (uint8_t)(t + 1);
-        x.sync();
         return true;
     }
 
@@ -1000,66 +979,157 @@ struct PlanEvaluator {
         return 0;
     }
 
-    // start rank of stage s (prefix sum of the group sizes, filled by set_groups)
+    // start rank of stage s (prefix sum of the group sizes, filled by begin)
     MB_HD int rank_start(int s) const { return w.rs[s]; }
 
-    MB_HD void set_groups(const uint8_t *row) {
-        int a = 0;
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = 0; s < pd.S; ++s) { w.gcode[s] = row[s]; w.rs[s] = (uint16_t)a; a += 1 << row[s]; }
-        w.rs[pd.S] = (uint16_t)a;
+    // ---- The per-stage cost model.  Each member computes one stage and returns its values in registers; the
+    // drivers (the methods below, CoopEvaluator in metis_coop.cuh) loop over the stages, store the values where
+    // they need them and do the order-dependent sums and the reductions.  A failing member returns METIS_FATAL_*
+    // with `aux` set for encode_error.
+
+    // one stage of StagePerformance.get_intra_stage_compute_performance (model/device_group.py:54-85) before the
+    // normalisation: 1 / the stage's execution time in p
+    MB_HD int stage_performance(int s, double &p) {
+        const int g = w.gcode[s], tpc = w.tpc[s];
+        const int a = rank_start(s), b = a + (1 << g);
+        int ta = 0, tb = 0;
+        if (!(ONE || T.p.num_types == 1)) { ta = type_of_rank(T, pd.ns, a); tb = type_of_rank(T, pd.ns, b - 1); }
+        p = 0.0;
+        if (ta != tb) return hetero_performance(a, b, 1 << (g - tpc), tpc, p);
+        const int bs = bs_total >> (g - tpc);
+        const int key = key_of(T, ta, tpc, bs);
+        if (key < 0) { aux = ((uint32_t)tpc << 16) | (uint32_t)bs; return METIS_FATAL_KEY_EXEC; }
+        if (T.exec_full[key] == 0.0) return METIS_FATAL_ZERODIV;
+        p = T.inv_exec[key];                                  // 1. / profile_cost
+        return 0;
     }
+
+    // one stage of LayerLoadBalancer._get_stage_memory_demand (model/load_balancer.py:29-55) for the partition in
+    // w.part, and its memory state (:57-63): capacity - demand
+    MB_HD int stage_memory(int s, double &demand, double &state) {
+        const bool one_type = ONE || T.p.num_types == 1;
+        const bool own_type = (T.p.corrected & METIS_FIX_Q6) != 0;
+        const int g = w.gcode[s], tpc = w.tpc[s];
+        const int a = rank_start(s), b = a + (1 << g);
+        int rc = 0;
+        demand = 0.001;
+        // opt-in METIS_FIX_Q6 (not the reference).  A single-type cluster skips it: memory_demand_own_type would take
+        // the plain branch's key (type0, the only type) and, like the !own_type below, raise no Q10 IndexError.
+        if (!ONE && own_type) {
+            rc = memory_demand_own_type(s, demand);
+        } else if (T.p.q10_devices < T.p.total_devices && !own_type && b > T.p.q10_devices) {
+            aux = 0;                                         // device_types[rank]: IndexError (load_balancer.py:36, Q10)
+            rc = METIS_FATAL_INDEX;
+        } else if (one_type || type_of_q10(T, pd.ns, a) == type_of_q10(T, pd.ns, b - 1)) {
+            const int bs = bs_total >> (g - tpc);
+            const int key = key_of(T, T.run_type[pd.ns * T.p.num_types], tpc, bs);
+            if (key < 0) { aux = ((uint32_t)tpc << 16) | (uint32_t)bs; rc = METIS_FATAL_KEY_MEMORY; }
+            else demand += range_sum<X>(T, kRangeMem, key, T.mem + (size_t)key * T.p.lpad, w.part[s], w.part[s + 1]) * kMemCoef;
+        } else {
+            rc = hetero_memory_demand(s, T.run_type[pd.ns * T.p.num_types], demand);
+        }
+        state = memory_capacity(a, b) - demand;
+        return rc;
+    }
+
+    // one stage of LayerLoadBalancer._adj_compute_performance (model/load_balancer.py:80-89) from its performance
+    // w.perf[s] and memory demand w.extra[s]: available_compute_capacity, adj_sc_capa and the stage's term of
+    // extra_required_capacity (0 for a stage within its memory)
+    MB_HD void stage_adjust(int s, double &avail, double &adj, double &extra) const {
+        const double c = w.perf[s], md = w.extra[s];
+        const double mc = memory_capacity(rank_start(s), rank_start(s) + group(s));
+        if (mc > md) {
+            adj = c;
+            avail = (c * mc / md) - c;
+            extra = 0.0;
+        } else {
+            avail = 0.0;
+            adj = c * (mc / md) * 0.9;
+            extra = c - adj;
+        }
+    }
+
+    // one stage of HeteroCostEstimator.get_cost (model/cost_estimator.py:175-233), in two members: the stage's
+    // execution time (_get_execution_cost :175-197) and its pp / dp / parameter update terms.  They are kept apart so
+    // that a driver can store the time before the terms are computed, which keeps the search kernels' register
+    // pressure where it was.  x / tp is evaluated as x * 2^-log2(tp) (same real quotient, same rounding); the
+    // remaining quotients come from the derived tables when the cluster has a single bandwidth value.
+    // returns true when the stage raises a KeyError
+    MB_HD bool stage_time(int s, double &len) {
+        const bool one_type = ONE || T.p.num_types == 1;
+        const int g = w.gcode[s], tpc = w.tpc[s];
+        const int a = one_type ? 0 : rank_start(s), b = a + (1 << g);
+        const int la = w.part[s], lb = w.part[s + 1];
+        const int ldp = g - tpc;
+        const int ta = one_type ? 0 : type_of_rank(T, pd.ns, a);
+        const int tb = one_type ? 0 : type_of_rank(T, pd.ns, b - 1);
+        len = 0.0;
+        if (ta != tb) return hetero_exec_cost(a, b, 1 << ldp, tpc, la, lb, len) != 0;
+        const int key = key_of(T, ta, tpc, bs_total >> ldp);
+        if (key < 0) return true;
+        len = range_sum<X>(T, kRangeLc, key, T.lc + (size_t)key * T.p.lpad, la, lb);
+        return false;
+    }
+
+    // pp term (0 for the last costed stage s = nstage - 1), dp term and parameter update term of stage s
+    MB_HD void stage_terms(int s, int nstage, double &pp, double &dpc, double &upd) const {
+        const int per = T.p.devices_per_node;
+        const int Lm = T.p.num_layers;
+        const bool ubw = T.p.uniform_bw != 0;
+        const int g = w.gcode[s], tpc = w.tpc[s];
+        const int la = w.part[s], lb = w.part[s + 1];
+        const int ldp = g - tpc;
+        const int mbs = bs_total >> ldp;
+        const double inv_tp = pow2_neg(tpc);                  // 1 / tp, exact power of two
+        pp = 0.0;
+        if (s < nstage - 1) {
+            if (ubw) {                                        // :224-227 via the derived tables
+                pp = (lb == Lm - 1) ? T.pp_vocab[mbs * T.p.num_tp + tpc] : T.pp_hidden[mbs];
+            } else {
+                double act;
+                if (lb == Lm - 1)
+                    act = (double)((int64_t)mbs * T.p.sequence_length * T.p.vocab_size) * inv_tp;
+                else
+                    act = (double)((int64_t)mbs * T.p.sequence_length * T.p.hidden_size);
+                pp = act / (bw_of_node_range(rank_start(s) / per, (rank_start(s + 2) - 1) / per) * 1048576.0);
+            }
+        }
+        // get_parameter_size_by_stage (model/activation_parameter.py:40-51)
+        int ntr = lb - la;
+        double params = 0.0;
+        if (la == 0) { params += T.p.input_params * inv_tp; --ntr; }
+        if (lb == Lm) { params += T.p.output_params * inv_tp; --ntr; }
+        params += T.p.transformer_params * inv_tp * (double)ntr;
+        if (ubw) dpc = T.dpk[ldp] * params;                   // :37-43
+        else {
+            const int dp = 1 << ldp;
+            dpc = (double)(2 * (dp - 1)) / ((double)dp * (dp_bandwidth(rank_start(s), dp, 1 << tpc) * 1048576.0)) * params;
+        }
+        upd = T.p.optimizer_time * inv_tp * T.ratio[lb - la];   // :145-147
+    }
+
+    // ---- Sequential drivers of the cost model (one plan per thread).
 
     // StagePerformance.get_intra_stage_compute_performance (model/device_group.py:54-85) -> w.perf
     MB_HD int compute_performance() {
-        const bool one_type = ONE || T.p.num_types == 1;
-        int fail = 0;
-        x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < pd.S; s += x.width()) {
-            const int g = w.gcode[s], tpc = w.tpc[s];
-            double p = 0.0;
-            if (one_type) {
-                const int bs = bs_total >> (g - tpc);
-                const int key = key_of(T, 0, tpc, bs);
-                if (key < 0) { aux = ((uint32_t)tpc << 16) | (uint32_t)bs; fail = METIS_FATAL_KEY_EXEC; }
-                else if (T.exec_full[key] == 0.0) fail = METIS_FATAL_ZERODIV;
-                else p = T.inv_exec[key];                     // 1. / profile_cost
-            } else {
-                const int a = rank_start(s), b = a + (1 << g);
-                const int ta = type_of_rank(T, pd.ns, a), tb = type_of_rank(T, pd.ns, b - 1);
-                if (ta == tb) {
-                    const int bs = bs_total >> (g - tpc);
-                    const int key = key_of(T, ta, tpc, bs);
-                    if (key < 0) { aux = ((uint32_t)tpc << 16) | (uint32_t)bs; fail = METIS_FATAL_KEY_EXEC; }
-                    else if (T.exec_full[key] == 0.0) fail = METIS_FATAL_ZERODIV;
-                    else p = T.inv_exec[key];
-                } else {
-                    const int rc = hetero_performance(a, b, 1 << (g - tpc), tpc, p);
-                    if (rc) fail = rc;
-                }
-            }
+        for (int s = 0; s < pd.S; ++s) {
+            double p;
+            const int rc = stage_performance(s, p);
             w.perf[s] = p;
-            w.extra[s] = fail ? (double)fail + (double)aux * 256.0 : 0.0;   // per-stage error mailbox (cooperative mode)
+            w.extra[s] = encode_error(rc, aux);
         }
-        x.sync();
         x.converge();
         PySum total;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int s = 0; s < pd.S; ++s) {                     // first failing stage in stage order, like the reference
-            if (w.extra[s] != 0.0) {
-                const uint64_t code = (uint64_t)w.extra[s];
-                aux = (uint32_t)(code >> 8);
-                return (int)(code & 0xFF);
-            }
+            if (w.extra[s] != 0.0) return decode_error(w.extra[s], aux);
             total.add(w.perf[s]);
         }
         const double tot = total.result();
         if (tot == 0.0) return METIS_FATAL_ZERODIV;
-        x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < pd.S; s += x.width()) w.perf[s] = w.perf[s] / tot;
-        x.sync();
+        for (int s = 0; s < pd.S; ++s) w.perf[s] = w.perf[s] / tot;
         return 0;
     }
 
@@ -1129,40 +1199,21 @@ struct PlanEvaluator {
     // in: w.perf (c_capa), w.extra (m_demand); out: w.perf; returns 1 = None, 0 ok, <0 fatal (negated code)
     MB_HD_NOINLINE int adjust_performance() {
         const int S = pd.S;
-        const bool one_type = ONE || T.p.num_types == 1;
         double *ratio = reinterpret_cast<double *>(w.subw);      // free after the vote (MAXL >= MAXS)
-        x.sync();
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < S; s += x.width()) {          // independent per stage (:80-89)
-            const int a = one_type ? 0 : rank_start(s), b = a + group(s);
-            const double c = w.perf[s], md = w.extra[s];
-            const double mc = one_type ? T.type_memory[0] * (double)group(s) : memory_capacity(a, b);
-            double av, adj;
-            if (mc > md) {
-                adj = c;
-                av = (c * mc / md) - c;
-            } else {
-                av = 0.0;
-                adj = c * (mc / md) * 0.9;
-            }
-            w.capa[s] = av;           // available_compute_capacity
-            w.mstate[s] = adj;        // adj_sc_capa
-        }
-        x.sync();
         double need = 0.;
         PySum avail_sum;
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = 0; s < S; ++s) {                            // order-dependent accumulations (:89-91)
-            const int a = one_type ? 0 : rank_start(s);
-            const double mc = one_type ? T.type_memory[0] * (double)group(s) : memory_capacity(a, a + group(s));
-            if (!(mc > w.extra[s])) need += (w.perf[s] - w.mstate[s]);
-            avail_sum.add(w.capa[s]);
+        for (int s = 0; s < S; ++s) {                            // :80-91, accumulated in stage order
+            double av, adj, extra;
+            stage_adjust(s, av, adj, extra);
+            w.capa[s] = av;           // available_compute_capacity
+            w.mstate[s] = adj;        // adj_sc_capa
+            need += extra;
+            avail_sum.add(av);
         }
         if (avail_sum.result() < need) return 1;
-        x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < S; s += x.width()) w.extra[s] = 0.;
-        x.sync();
+        for (int s = 0; s < S; ++s) w.extra[s] = 0.;
         int guard = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
         while (need > 0.01) {
@@ -1170,11 +1221,9 @@ struct PlanEvaluator {
 #pragma unroll (X::kUniform ? 1 : 0)
             for (int s = 0; s < S; ++s) tot.add(w.capa[s] > 0.001 ? w.perf[s] : 0.0);
             const double tmp_total = tot.result();
-            x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
-            for (int s = x.lane(); s < S; s += x.width())        // c_capa_ratio list (:98), before the updates
+            for (int s = 0; s < S; ++s)                          // c_capa_ratio list (:98), before the updates
                 ratio[s] = w.capa[s] > 0.001 ? w.perf[s] / tmp_total : 0.0;
-            x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
             for (int s = 0; s < S; ++s) {                        // :100-104, sequential: `need` changes as it goes
                 const double av = w.capa[s];
@@ -1186,10 +1235,8 @@ struct PlanEvaluator {
             }
             if (++guard > 4096) return -METIS_FATAL_HANG;
         }
-        x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < S; s += x.width()) w.perf[s] = w.extra[s] + w.mstate[s];
-        x.sync();
+        for (int s = 0; s < S; ++s) w.perf[s] = w.extra[s] + w.mstate[s];
         return 0;
     }
 
@@ -1201,53 +1248,25 @@ struct PlanEvaluator {
     // call is skipped here.
     MB_HD int memory_phase(int attempt) {
         const int S = pd.S;
-        const bool one_type = ONE || T.p.num_types == 1;
-        const int type0 = T.run_type[pd.ns * T.p.num_types];
-        const bool q10_short = T.p.q10_devices < T.p.total_devices;   // node 0 has fewer GPUs than the average (Q10)
-        const bool own_type = (T.p.corrected & METIS_FIX_Q6) != 0;
-        x.sync();                                            // balance_run's last readers of capa/extra/mstate are done
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < S; s += x.width()) {
-            const int g = w.gcode[s], tpc = w.tpc[s];
-            const int a = (one_type && !q10_short) ? 0 : rank_start(s), b = a + (1 << g);
-            double md = 0.001, err = 0.0;
-            if (own_type) {                                  // opt-in METIS_FIX_Q6 (not the reference)
-                const int rc = memory_demand_own_type(s, md);
-                if (rc) err = (double)rc + (double)aux * 256.0;
-            } else if (q10_short && b > T.p.q10_devices) {
-                err = (double)METIS_FATAL_INDEX;             // device_types[rank]: IndexError (load_balancer.py:36, Q10)
-            } else if (one_type || type_of_q10(T, pd.ns, a) == type_of_q10(T, pd.ns, b - 1)) {
-                const int bs = bs_total >> (g - tpc);
-                const int key = key_of(T, type0, tpc, bs);
-                if (key < 0) err = (double)METIS_FATAL_KEY_MEMORY + (double)(((uint32_t)tpc << 16) | (uint32_t)bs) * 256.0;
-                else md += range_sum<X>(T, kRangeMem, key, T.mem + (size_t)key * T.p.lpad, w.part[s], w.part[s + 1]) * kMemCoef;
-            } else {
-                const int rc = hetero_memory_demand(s, type0, md);
-                if (rc) err = (double)rc + (double)aux * 256.0;
-            }
+        for (int s = 0; s < S; ++s) {
+            double md, state;
+            const int rc = stage_memory(s, md, state);
             w.extra[s] = md;
-            const double mc = one_type ? T.type_memory[0] * (double)(1 << g) : memory_capacity(rank_start(s), rank_start(s) + (1 << g));
-            w.capa[s] = mc - md;
-            w.mstate[s] = err;
-            if (tap) { tap->demand[s] = md; tap->state[s] = mc - md; }
+            w.capa[s] = state;
+            w.mstate[s] = encode_error(rc, aux);
+            if (tap) { tap->demand[s] = md; tap->state[s] = state; }
         }
-        x.sync();
         x.converge();
         bool oom = false;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int s = 0; s < S; ++s) {
-            if (w.mstate[s] != 0.0) {
-                const uint64_t code = (uint64_t)w.mstate[s];
-                aux = (uint32_t)(code >> 8);
-                return -(int)(code & 0xFF);
-            }
+            if (w.mstate[s] != 0.0) return -decode_error(w.mstate[s], aux);
             if (w.capa[s] < 0) oom = true;
         }
         if (!oom) {
-            x.sync();
 #pragma unroll (X::kUniform ? 1 : 0)
-            for (int s = x.lane(); s < S; s += x.width()) w.mstate[s] = w.capa[s];
-            x.sync();
+            for (int s = 0; s < S; ++s) w.mstate[s] = w.capa[s];
             return 1;
         }
         if (attempt >= 3) return 0;
@@ -1369,88 +1388,31 @@ struct PlanEvaluator {
     }
 
     // HeteroCostEstimator.get_cost (model/cost_estimator.py:199-244); returns 0 ok, 1 KeyError.
-    // x / tp is evaluated as x * 2^-log2(tp) (same real quotient, same rounding); the remaining
-    // quotients come from the derived tables when the cluster has a single bandwidth value.
     MB_HD int get_cost(double &cost_out) {
-        const int per = T.p.devices_per_node;
-        const int Lm = T.p.num_layers;
         const bool one_type = ONE || T.p.num_types == 1;
-        const bool ubw = T.p.uniform_bw != 0;
         const int nstage = pd.label < pd.S ? pd.label : pd.S;  // zip(range(plan.num_stage), strategies)
         // rank_node_map holds num_nodes * devices(node 0) ranks (cluster_bandwidth.py:34-47, Q10): a costed stage
         // (or its pipeline successor) beyond that raises KeyError -> the candidate is skipped
         if (T.p.q10_devices < T.p.total_devices && rank_start(nstage) > T.p.q10_devices) return 1;
-        // execution time of every stage first (independent range sums; w.capa[s] = time, w.extra[s] = error flag)
-        x.sync();
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < nstage; s += x.width()) {
-            const int g = w.gcode[s], tpc = w.tpc[s];
-            const int a = one_type ? 0 : rank_start(s), b = a + (1 << g);
-            const int la = w.part[s], lb = w.part[s + 1];
-            const int ldp = g - tpc;
-            const int ta = one_type ? 0 : type_of_rank(T, pd.ns, a);
-            const int tb = one_type ? 0 : type_of_rank(T, pd.ns, b - 1);
-            double len = 0.0, err = 0.0;
-            if (ta == tb) {                                   // _get_execution_cost :175-188
-                const int key = key_of(T, ta, tpc, bs_total >> ldp);
-                if (key < 0) err = 1.0;
-                else len = range_sum<X>(T, kRangeLc, key, T.lc + (size_t)key * T.p.lpad, la, lb);
-            } else if (hetero_exec_cost(a, b, 1 << ldp, tpc, la, lb, len)) {
-                err = 1.0;
-            }
-            w.capa[s] = len;
-            w.extra[s] = err;
-        }
-        x.sync();
+        // execution time of every stage first (w.capa[s]); the terms only when no stage raised a KeyError
         bool bad = false;
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < nstage; s += x.width()) bad = bad || (w.extra[s] != 0.0);
-        if (x.any(bad)) return 1;                             // KeyError raised while costing a stage
+        for (int s = 0; s < nstage; ++s) {
+            double len;
+            if (stage_time(s, len)) bad = true;
+            w.capa[s] = len;
+        }
+        if (bad) return 1;                                    // KeyError raised while costing a stage
         double *ppterm = reinterpret_cast<double *>(w.subw);  // free after the vote (MAXL >= MAXS)
         double max_len = -INFINITY, max_upd = -INFINITY, max_dp = -INFINITY;
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = x.lane(); s < nstage; s += x.width()) {  // independent per-stage terms
-            const int g = w.gcode[s], tpc = w.tpc[s];
-            const int la = w.part[s], lb = w.part[s + 1];
-            const int ldp = g - tpc;
-            const int mbs = bs_total >> ldp;
-            const double inv_tp = pow2_neg(tpc);              // 1 / tp, exact power of two
+        for (int s = 0; s < nstage; ++s) {
+            double dpc, upd;
+            stage_terms(s, nstage, ppterm[s], dpc, upd);
             if (w.capa[s] > max_len) max_len = w.capa[s];
-            double pp = 0.0;
-            if (s < nstage - 1) {
-                if (ubw) {                                    // :224-227 via the derived tables
-                    pp = (lb == Lm - 1) ? T.pp_vocab[mbs * T.p.num_tp + tpc] : T.pp_hidden[mbs];
-                } else {
-                    double act;
-                    if (lb == Lm - 1)
-                        act = (double)((int64_t)mbs * T.p.sequence_length * T.p.vocab_size) * inv_tp;
-                    else
-                        act = (double)((int64_t)mbs * T.p.sequence_length * T.p.hidden_size);
-                    const int a = rank_start(s), b2 = rank_start(s + 2);
-                    pp = act / (bw_of_node_range(a / per, (b2 - 1) / per) * 1048576.0);
-                }
-            }
-            ppterm[s] = pp;
-            // get_parameter_size_by_stage (model/activation_parameter.py:40-51)
-            int ntr = lb - la;
-            double params = 0.0;
-            if (la == 0) { params += T.p.input_params * inv_tp; --ntr; }
-            if (lb == Lm) { params += T.p.output_params * inv_tp; --ntr; }
-            params += T.p.transformer_params * inv_tp * (double)ntr;
-            double dpc;                                       // :37-43
-            if (ubw) dpc = T.dpk[ldp] * params;
-            else {
-                const int dp = 1 << ldp;
-                dpc = (double)(2 * (dp - 1)) / ((double)dp * (dp_bandwidth(rank_start(s), dp, 1 << tpc) * 1048576.0)) * params;
-            }
             if (dpc > max_dp) max_dp = dpc;
-            const double upd = T.p.optimizer_time * inv_tp * T.ratio[lb - la];   // :145-147
             if (upd > max_upd) max_upd = upd;
         }
-        max_len = x.max_all(max_len);
-        max_upd = x.max_all(max_upd);
-        max_dp = x.max_all(max_dp);
-        x.sync();
         PySum lens_sum;                                       // order-dependent sums, stage order
         double pp_cost = 0., fb_sync = 0.;
 #pragma unroll (X::kUniform ? 1 : 0)
