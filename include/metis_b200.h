@@ -183,7 +183,10 @@ void metis_set_profile_events(void *before_kernel, void *after_kernel);
 
 /* Bytes of device scratch metis_het_search needs for a shard of `num_plans` plans: the packed tables
  * plus two lists of 16 B per plan (worst case: every plan has a valid strategy); `max_stage` is ignored.
- * metis_het_detail / metis_homo_cost need metis_het_workspace_bytes(problem, 0, 1). */
+ * metis_het_detail / metis_homo_cost need metis_het_workspace_bytes(problem, 0, 1).
+ * About 36 B per plan in all: a space whose workspace, rows and records do not fit the device (or that has 2^32
+ * plans or 4 GiB of rows) is searched in ordinal windows, each a MetisPlanSpace of its own
+ * (metis_b200.flatten.plan_windows sizes them with this function). */
 int64_t metis_het_workspace_bytes(const MetisProblem *problem, int64_t num_plans, int32_t max_stage);
 
 /*

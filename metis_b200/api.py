@@ -224,36 +224,36 @@ class HetSearchResult(Sequence):
         """argmin (cost, position): the first entry of the ranked list.  The search kernels reduce it on the device
         (het_finalize_kernel: lowest cost, then lowest ordinal, then lowest step), so no sort is needed for it."""
         if self.rank_order is None and self._best_key is not None and len(self):
-            rec = self.candidates.records                     # sorted by (ordinal, step): bisect, no temporaries
-            want = (int(self._best_key[0]), int(self._best_key[1]))
-            lo, hi = 0, len(rec)
-            while lo < hi:
-                mid = (lo + hi) >> 1
-                r = rec[mid]
-                if (int(r['ordinal']), int(r['step'])) < want:
-                    lo = mid + 1
-                else:
-                    hi = mid
-            if lo < len(rec) and (int(rec[lo]['ordinal']), int(rec[lo]['step'])) == want:
-                return self.candidates.tuples([lo])[0]
+            at = self.candidates.index_of(*self._best_key)    # records sorted by (ordinal, step): no temporaries
+            if at is not None:
+                return self.candidates.tuples([at])[0]
         top = self.ranked(1)
         return top[0] if top else None
 
 
 def het_problem(args, gpu_cluster, profile_data, model_config, layer_load_balancer=None,
                 node_sequences: Optional[Sequence[Sequence]] = None, corrected: Sequence[str] = (),
-                rows_out: Optional[np.ndarray] = None, device_rows: bool = False):
+                rows_out: Optional[np.ndarray] = None, device_rows: bool = False, unbounded: bool = False):
     """Flatten the inputs of cost_het_cluster() (order of ``set(device_types)`` = quirk Q4).  ``device_rows``: the
-    host lists only the compositions, the GPU writes the device-group rows (SURVEY.md 8(f)-1)."""
+    host lists only the compositions, the GPU writes the device-group rows (SURVEY.md 8(f)-1).  ``unbounded`` (with
+    ``device_rows``): a space beyond the limits of one search is returned too, for a windowed search."""
     if node_sequences is None:
         node_sequences = list(permutations(set(gpu_cluster.get_device_types())))
     norm = layer_load_balancer.norm_layer_duration if layer_load_balancer is not None else None
     problem = flatten.build_problem(profile_data, gpu_cluster, model_config, args.gbs,
                                     args.max_profiled_tp_degree, args.max_profiled_batch_size, node_sequences,
                                     norm, corrected=corrected)
-    space = flatten.build_plan_space(len(node_sequences), gpu_cluster.get_total_num_devices(), args.gbs,
-                                     args.num_layers, args.min_group_scale_variance, args.max_permute_len,
-                                     corrected=corrected, rows_out=rows_out, device_rows=device_rows)
+    space = None
+    if device_rows and unbounded:
+        space = flatten.build_device_plan_space(len(node_sequences), gpu_cluster.get_total_num_devices(), args.gbs,
+                                                args.num_layers, args.min_group_scale_variance, args.max_permute_len,
+                                                corrected=corrected)
+        # None: a composition has more merged groups than the row kernel handles, so the rows come from the host
+        device_rows = False
+    if space is None:
+        space = flatten.build_plan_space(len(node_sequences), gpu_cluster.get_total_num_devices(), args.gbs,
+                                         args.num_layers, args.min_group_scale_variance, args.max_permute_len,
+                                         corrected=corrected, rows_out=rows_out, device_rows=device_rows)
     return problem, space, [tuple(s) for s in node_sequences]
 
 
@@ -315,8 +315,11 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     dev = search._require_cuda(device)
     # the host lists the compositions (a few thousand records); the rows themselves are written by the GPU
     problem, space, seqs = het_problem(args, gpu_cluster, profile_data, model_config, layer_load_balancer,
-                                       node_sequences, corrected=tuple(corrected), device_rows=True)
+                                       node_sequences, corrected=tuple(corrected), device_rows=True, unbounded=True)
     t1 = time.perf_counter()
+    windows = _het_windows(problem, space, dev, rank, world)
+    if windows is not None:
+        return _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1)
     stride = 3 * int(space.blocks['num_stage'].max()) + 1
     dp, searcher = _engine(problem, space, dev, rank, world, stride)
     dp.upload()
@@ -352,9 +355,99 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     # sorted(result, key=cost) is the CALLER's step in the reference (cost_het_cluster.py:76): its permutation is
     # computed by the device sort when ranked() is first asked for; best() needs no sort at all
     result = HetSearchResult(cand, out.rank_order,
-                             dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected))),
+                             dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)), num_windows=1),
                              ranker=search.make_ranker(searcher, out.records_dev) if len(out.records) else None,
                              best_key=(best[1], best[2]) if best else None)
+    result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
+                      'decode_columns_s': time.perf_counter() - t2}
+    return result
+
+
+# A space whose search needs less device memory than this (and is within the 32-bit limits of one search) is searched
+# in one window without asking the device how much memory is free.
+_ONE_SEARCH_BYTES = 1 << 31
+# Below this budget a windowed search is refused: its windows would be so small that reloading them dominates.
+_MIN_WINDOW_BYTES = 1 << 30
+
+
+def _engine_bytes(key) -> int:
+    """Device bytes held by the cached one-search engine ``key`` (reusable by the search being planned)."""
+    eng = _ENGINES.get(key)
+    if eng is None:
+        return 0
+    dp, searcher = eng
+    held = dp._dev.numel()
+    for t in (searcher.workspace, searcher.records, searcher.detail, searcher._sort_ws):
+        if t is not None:
+            held += t.numel() * t.element_size()
+    return held
+
+
+def _het_windows(problem, space, dev, rank: int, world: int):
+    """None when ``space`` is searched by one metis_het_search call (today's path, the cached engine untouched), else
+    its windows (flatten.plan_windows), sized from the device memory free for them.  Every rank takes the smallest
+    budget of all ranks, so that all ranks make the same choice and cut the same windows."""
+    from . import search
+    if space.comp_recs is None:                               # host rows: build_plan_space kept its limits
+        return None
+    per_plan, per_row, per_rec, fixed = search.window_cost_model(problem)
+    shard = -(-space.num_plans // world) + 128                # plans of one rank's shard, with a tile of slack
+    need = shard * per_plan + int(space.rows_total_bytes) * per_row + len(space.comp_recs) * per_rec
+    if flatten.fits_one_search(space) and need + fixed < _ONE_SEARCH_BYTES:
+        return None
+    key = (dev.index if dev.index is not None else -1, rank, world)
+    held = _engine_bytes(key)
+    if flatten.fits_one_search(space) and need + fixed <= held and world == 1:
+        return None                                           # the cached engine already holds such a search
+    # the cached engine's buffers are reused by a one-window search and freed for a windowed one: both count as free
+    budget = search.agree_budget(search.window_budget(dev, fixed) + held, dev)
+    if flatten.fits_one_search(space) and need <= budget:
+        return None
+    if budget < _MIN_WINDOW_BYTES:
+        raise native.MetisNativeError(
+            f'{max(budget, 0) / 2 ** 20:.0f} MiB of device memory are free for a search of {space.num_plans} plans; '
+            f'searching it in windows needs at least {_MIN_WINDOW_BYTES >> 20} MiB')
+    _ENGINES.pop(key, None)
+    import torch
+    torch.cuda.empty_cache()
+    # a rank searches 1/world of each window's plans; the rows and composition records are whole on every rank
+    return flatten.plan_windows(space, budget, per_plan / world, per_row, per_rec)
+
+
+def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int, dist, corrected, t0: float,
+                      t1: float) -> HetSearchResult:
+    """cost_het_cluster() for a space larger than one search: flatten.plan_windows' windows, searched in ordinal order
+    (search.search_windows), merged on the host; the result keeps the records only (search.WindowedCandidates)."""
+    from . import search
+    failure = merged = searcher = None
+    try:
+        merged, _dp, searcher = search.search_windows(problem, windows, dev, rank, world)
+    except Exception as exc:                                  # noqa: BLE001 - re-raised below on every rank
+        if not dist:
+            raise
+        failure = exc
+    if dist:
+        summary, best = search.global_exchange(merged.summary if merged is not None else {},
+                                               merged.best if merged is not None else None, dev, int(failure is not None))
+        if summary['any_rank_failed']:
+            raise failure if failure is not None else native.MetisNativeError('the search failed on another rank')
+        if summary['global_fatal_ordinal'] < 2 ** 62:
+            summary.update(fatal_ordinal=summary['global_fatal_ordinal'], fatal_code=summary['global_fatal_code'],
+                           fatal_aux=summary['global_fatal_aux'])
+        else:
+            summary['fatal_ordinal'] = 2 ** 64 - 1
+            merged = search.gather_window_records(merged, dev)
+    else:
+        summary, best = merged.summary, merged.best
+    if summary['fatal_ordinal'] != 2 ** 64 - 1:
+        search.raise_fatal(summary, problem)                  # the reference dies at that plan (quirk Q8)
+    t2 = time.perf_counter()
+    cand = search.WindowedCandidates(merged.records, merged.bases, merged.firsts, windows, problem, seqs, searcher)
+    result = HetSearchResult(cand, None, dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)),
+                                              num_windows=len(windows)),
+                             best_key=(best[1], best[2]) if best else None)
+    if len(merged.records):
+        result._ranker = search.make_window_ranker(searcher, merged.records, result.summary)
     result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
                       'decode_columns_s': time.perf_counter() - t2}
     return result

@@ -362,22 +362,11 @@ def build_plan_space(num_node_sequences: int, num_devices: int, gbs: int, num_la
     lib = lib or native.load_library()
     batches = [b for b in range(gbs, 0, -1) if gbs % b == 0]   # plan.py:120-124
     if device_rows:
-        counts, recs, pool, most = enumerate_compositions(1, cap + 1, num_devices, variance, max_permute_len, lib)
-        if most <= native.METIS_MAX_PERMUTE_GROUPS:
-            offsets, off = {}, 0
-            for stages in range(1, cap + 2):
-                offsets[stages] = off
-                off += int(counts[stages - 1]) * stages
-            nrows_of = lambda st: int(counts[st - 1]) if 1 <= st <= cap + 1 else 0     # noqa: E731
-            plan_blocks = _walk_blocks(num_node_sequences, cap, nrows_of, corrected)
-            _check_stage_limit(plan_blocks)
-            blocks, total = _blocks_array(plan_blocks, nrows_of, lambda st: offsets[st], len(batches))
-            if off > 0xFFFFFFFF or total > 0xFFFFFFF0:
+        space = build_device_plan_space(num_node_sequences, num_devices, gbs, num_layers, variance, max_permute_len,
+                                        lib, corrected)
+        if space is not None:
+            if not fits_one_search(space):
                 raise NotImplementedError('device-group tables of 4 GiB or more / more than 2^32 plans are not supported')
-            space = FlatPlanSpace(total, blocks, np.asarray(batches, dtype=np.int32), np.zeros(0, dtype=np.uint8))
-            space.rows_total_bytes = off
-            space.comp_recs, space.comp_pool = recs, pool
-            space.tables = _LazyTables(cap, num_devices, variance, max_permute_len)
             return space
         # a composition with more merged groups than the device kernel handles: enumerate on the host
     cache: Dict[int, np.ndarray] = enumerate_device_group_tables(1, cap + 1, num_devices, variance, max_permute_len, lib,
@@ -423,6 +412,233 @@ class _LazyTables(dict):
     def __contains__(self, key):
         self._fill()
         return dict.__contains__(self, key)
+
+
+# One search holds at most this many plans (a list entry and a record carry the ordinal in 32 bits) and rows of
+# less than 4 GiB (a list entry addresses its row with a 32-bit byte offset).
+MAX_SEARCH_PLANS = 0xFFFFFFF0
+MAX_SEARCH_ROW_BYTES = 0xFFFFFFFF
+
+
+def fits_one_search(space: FlatPlanSpace) -> bool:
+    """Whether ``space`` is within the 32-bit limits of one metis_het_search call."""
+    return space.num_plans <= MAX_SEARCH_PLANS and int(space.rows_total_bytes) <= MAX_SEARCH_ROW_BYTES
+
+
+def build_device_plan_space(num_node_sequences: int, num_devices: int, gbs: int, num_layers: int, variance,
+                            max_permute_len: int, lib=None, corrected: Sequence[str] = ()) -> Optional[FlatPlanSpace]:
+    """The whole candidate space as a device_rows space (compositions listed on the host, rows written by the GPU),
+    WITHOUT the limits of one search: the input of plan_windows.  None when a composition has more merged groups than
+    the row kernel handles (such spaces are enumerated on the host by build_plan_space)."""
+    cap = min(num_devices, num_layers)
+    lib = lib or native.load_library()
+    batches = [b for b in range(gbs, 0, -1) if gbs % b == 0]   # plan.py:120-124
+    counts, recs, pool, most = enumerate_compositions(1, cap + 1, num_devices, variance, max_permute_len, lib)
+    if most > native.METIS_MAX_PERMUTE_GROUPS:
+        return None
+    offsets, off = {}, 0
+    for stages in range(1, cap + 2):
+        offsets[stages] = off
+        off += int(counts[stages - 1]) * stages
+    nrows_of = lambda st: int(counts[st - 1]) if 1 <= st <= cap + 1 else 0     # noqa: E731
+    plan_blocks = _walk_blocks(num_node_sequences, cap, nrows_of, corrected)
+    _check_stage_limit(plan_blocks)
+    blocks, total = _blocks_array(plan_blocks, nrows_of, lambda st: offsets[st], len(batches))
+    space = FlatPlanSpace(total, blocks, np.asarray(batches, dtype=np.int32), np.zeros(0, dtype=np.uint8))
+    space.rows_total_bytes = off
+    space.comp_recs, space.comp_pool = recs, pool
+    space.tables = _LazyTables(cap, num_devices, variance, max_permute_len)
+    return space
+
+
+@dataclass
+class PlanWindow:
+    """A contiguous ordinal range of a larger space, as a space of its own: global ordinal = ``base`` + the window's
+    ordinal.  Its blocks cover whole composition slices (METIS_COMP_SLICE_ROWS rows) of the parent's blocks; row r of
+    window block b is row ``row_base[b] + r`` of the parent's block.  The window's rows are the union of the row ranges
+    its blocks cover, per stage count (node sequences share them), written by metis_generate_rows from ``comp_recs``."""
+    base: int
+    space: FlatPlanSpace
+    row_base: np.ndarray          # int64 per window block
+
+    def plan_at(self, ordinal: int) -> Tuple[int, int, int, int, int, int]:
+        """Global ``ordinal`` -> (ns_idx, label_stage, dg_idx, batches, num_stage, byte offset of its row in the
+        window's rows); dg_idx is the row in the whole space's table of that stage count, as in InterStagePlan."""
+        sp = self.space
+        rel = ordinal - self.base
+        if not 0 <= rel < sp.num_plans:
+            raise IndexError(f'ordinal {ordinal} is not in this window')
+        b = int(np.searchsorted(sp.blocks['first_ordinal'], rel, side='right')) - 1
+        blk = sp.blocks[b]
+        row, div = divmod(rel - int(blk['first_ordinal']), len(sp.batches))
+        S = int(blk['num_stage'])
+        return (int(blk['ns_idx']), int(blk['label_stage']), int(self.row_base[b]) + row, int(sp.batches[div]), S,
+                int(blk['rows_offset']) + row * S)
+
+    def locate(self, ordinal: int, rows: np.ndarray) -> Tuple[int, int, int, int, np.ndarray]:
+        """Global ``ordinal`` -> (ns_idx, label_stage, dg_idx, batches, device_groups) like FlatPlanSpace.locate, with
+        the codes read from ``rows`` (the window's row blob, e.g. generated on the host)."""
+        ns, label, dg, batches, S, at = self.plan_at(ordinal)
+        return ns, label, dg, batches, rows[at:at + S]
+
+
+def window_bytes(space: FlatPlanSpace, plan_bytes: float, row_bytes: float, rec_bytes: float) -> float:
+    """Device memory of searching ``space`` under the cost model of plan_windows."""
+    return space.num_plans * plan_bytes + int(space.rows_total_bytes) * row_bytes + len(space.comp_recs) * rec_bytes
+
+
+def _slices_by_stage(space: FlatPlanSpace) -> Dict[int, Tuple[int, np.ndarray]]:
+    """S -> (index of the first composition record of S, row boundaries of its slices: K+1 int64 values, 0 .. rows)."""
+    recs = space.comp_recs
+    st = recs['stages'].astype(np.int64)
+    out = {}
+    for S in np.unique(space.blocks['num_stage']).tolist():
+        lo, hi = int(np.searchsorted(st, S, side='left')), int(np.searchsorted(st, S, side='right'))
+        first = (recs['row_offset'][lo:hi] - recs['row_offset'][lo]) // S
+        nrows = int(space.blocks['num_rows'][space.blocks['num_stage'] == S][0])
+        out[S] = (lo, np.append(first, nrows).astype(np.int64))
+    return out
+
+
+def _uncovered(k0: int, c: np.ndarray, bounds: np.ndarray, covered: List[Tuple[int, int]]):
+    """For slice ranges [k0, c) (c an array): slices and rows not yet in ``covered`` (disjoint slice intervals)."""
+    new_k = c - k0
+    new_r = bounds[c] - bounds[k0]
+    for a, b in covered:
+        lo = max(k0, a)
+        hi = np.minimum(c, b)
+        hit = hi > lo
+        new_k = new_k - np.where(hit, hi - lo, 0)
+        new_r = new_r - np.where(hit, bounds[np.where(hit, hi, lo)] - bounds[lo], 0)
+    return new_k, new_r
+
+
+def arena_bytes(windows: Sequence[PlanWindow], plan_bytes: float, row_bytes: float, rec_bytes: float) -> float:
+    """Device memory of searching ``windows`` one after the other in one arena and workspace sized for all of them:
+    the most plans, the most rows and the most composition records of any window, under window_bytes' cost model."""
+    return (max(w.space.num_plans for w in windows) * plan_bytes
+            + max(int(w.space.rows_total_bytes) for w in windows) * row_bytes
+            + max(len(w.space.comp_recs) for w in windows) * rec_bytes)
+
+
+def plan_windows(space: FlatPlanSpace, budget: float, plan_bytes: float = 1.0, row_bytes: float = 0.0,
+                 rec_bytes: float = 0.0) -> List[PlanWindow]:
+    """Cut a device_rows space (build_device_plan_space) into windows, in ordinal order, each within the limits of one
+    search (fewer than 2^32 plans, rows below 4 GiB), such that one arena and workspace sized for all of them fit
+    ``budget`` bytes of device memory (arena_bytes), counted as ``plan_bytes`` per plan, ``row_bytes`` per byte of
+    rows and ``rec_bytes`` per composition record.  Cuts fall on composition slices; a window holds at least one
+    slice, whatever the budget."""
+    target = budget
+    for _ in range(8):
+        windows = _cut_windows(space, target, plan_bytes, row_bytes, rec_bytes)
+        peak = arena_bytes(windows, plan_bytes, row_bytes, rec_bytes)
+        if peak <= budget or target <= 0:
+            break
+        # the window with the most plans and the one with the most rows differ: cut every window smaller
+        target = min(target * budget / peak, target - 1)
+    return windows
+
+
+def _cut_windows(space: FlatPlanSpace, budget: float, plan_bytes: float, row_bytes: float,
+                 rec_bytes: float) -> List[PlanWindow]:
+    """Greedy cut of plan_windows: each window on its own within ``budget`` (window_bytes)."""
+    if space.comp_recs is None:
+        raise NotImplementedError('only spaces whose rows the GPU writes (device_rows) can be searched in windows')
+    ndiv = len(space.batches)
+    slices = _slices_by_stage(space)
+    windows: List[PlanWindow] = []
+    seg: List[Tuple[int, int, int]] = []                  # (parent block, first slice, end slice)
+    covered: Dict[int, List[Tuple[int, int]]] = {}        # S -> disjoint slice intervals of the window's rows
+    state = [0, 0, 0, 0]                                  # plans, row bytes, records, base ordinal
+
+    def close():
+        windows.append(_make_window(space, slices, seg, covered, state[3]))
+        state[3] += state[0]
+        state[:3] = [0, 0, 0]
+        seg.clear()
+        covered.clear()
+
+    def add(b, S, k0, k1, bounds):
+        nk, nr = _uncovered(k0, np.asarray([k1]), bounds, covered.get(S, []))
+        state[0] += int(bounds[k1] - bounds[k0]) * ndiv
+        state[1] += int(nr[0]) * S
+        state[2] += int(nk[0])
+        seg.append((b, k0, k1))
+        ivs = sorted(covered.get(S, []) + [(k0, k1)])
+        merged = [ivs[0]]
+        for a, e in ivs[1:]:
+            if a <= merged[-1][1]:
+                merged[-1] = (merged[-1][0], max(merged[-1][1], e))
+            else:
+                merged.append((a, e))
+        covered[S] = merged
+
+    for b in range(len(space.blocks)):
+        S = int(space.blocks['num_stage'][b])
+        bounds = slices[S][1]
+        K = len(bounds) - 1
+        k0 = 0
+        while k0 < K:
+            span, fit = 256, k0
+            while True:                                   # largest end slice that fits, probing a growing span
+                c = np.arange(k0 + 1, min(K, k0 + span) + 1, dtype=np.int64)
+                nk, nr = _uncovered(k0, c, bounds, covered.get(S, []))
+                plans = state[0] + (bounds[c] - bounds[k0]) * ndiv
+                rows = state[1] + nr * S
+                cost = plans * plan_bytes + rows * row_bytes + (state[2] + nk) * rec_bytes
+                ok = (plans <= MAX_SEARCH_PLANS) & (rows <= MAX_SEARCH_ROW_BYTES) & (cost <= budget)
+                n_ok = int(np.argmin(ok)) if not ok.all() else len(ok)
+                if n_ok:
+                    fit = int(c[n_ok - 1])
+                if n_ok < len(ok) or c[-1] == K:
+                    break
+                span *= 4
+            if fit == k0:
+                if seg:                                   # nothing more fits: the next window starts here
+                    close()
+                    continue
+                fit = k0 + 1                              # an empty window takes one slice
+            add(b, S, k0, fit, bounds)
+            k0 = fit
+            if k0 < K:
+                close()
+    if seg:
+        close()
+    return windows
+
+
+def _make_window(space: FlatPlanSpace, slices, seg, covered, base: int) -> PlanWindow:
+    ndiv = len(space.batches)
+    recs = space.comp_recs
+    at: Dict[Tuple[int, int], int] = {}                   # (S, interval start) -> byte offset in the window's rows
+    parts, off = [], 0
+    for S in sorted(covered):
+        lo, bounds = slices[S]
+        for a, e in covered[S]:
+            at[(S, a)] = off
+            part = recs[lo + a:lo + e].copy()
+            part['row_offset'] = part['row_offset'] - part['row_offset'][0] + off
+            parts.append(part)
+            off += int(bounds[e] - bounds[a]) * S
+    blocks = np.zeros(len(seg), dtype=native.BLOCK_DTYPE)
+    row_base = np.zeros(len(seg), dtype=np.int64)
+    ordinal = 0
+    for i, (b, k0, k1) in enumerate(seg):
+        src = space.blocks[b]
+        S = int(src['num_stage'])
+        bounds = slices[S][1]
+        a = next(a for a, e in covered[S] if a <= k0 and k1 <= e)
+        blocks[i] = src
+        blocks[i]['first_ordinal'] = ordinal
+        blocks[i]['rows_offset'] = at[(S, a)] + int(bounds[k0] - bounds[a]) * S
+        blocks[i]['num_rows'] = int(bounds[k1] - bounds[k0])
+        row_base[i] = bounds[k0]
+        ordinal += int(bounds[k1] - bounds[k0]) * ndiv
+    w = FlatPlanSpace(ordinal, blocks, space.batches, np.zeros(0, dtype=np.uint8))
+    w.rows_total_bytes = off
+    w.comp_recs = np.concatenate(parts) if parts else recs[:0].copy()
+    w.comp_pool = space.comp_pool
+    return PlanWindow(base, w, row_base)
 
 
 def enumerate_compositions(first_stage: int, last_stage: int, num_gpus: int, variance, max_permute_len: int, lib=None):

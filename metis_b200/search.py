@@ -43,13 +43,20 @@ class DeviceProblem:
     host -> device copy; ``reload`` puts another problem / space of compatible size into the same buffers."""
 
     def __init__(self, problem: flatten.FlatProblem, space: flatten.FlatPlanSpace, device=None,
-                 pinned: bool = True, rows_capacity: int = 0):
+                 pinned: bool = True, rows_capacity: int = 0, reserve: Sequence[flatten.FlatPlanSpace] = ()):
+        """``reserve``: further spaces (the windows of a windowed search) the arena is sized for up front, so that
+        reloading any of them reuses the buffers."""
         self.device = _require_cuda(device)
         self.lib = native.load_library()
         self.pinned = pinned
         self._host = self._dev = None
         self._off: Dict[str, Tuple[int, int]] = {}           # name -> (offset, capacity)
         self._used: Dict[str, int] = {}
+        self._reserve: Dict[str, int] = {}
+        for s in reserve:
+            flat = self._arrays(problem, s)
+            for name in _ARENA_ORDER:
+                self._reserve[name] = max(self._reserve.get(name, 0), self._need(flat, s, name))
         self._allocate(self._arrays(problem, space), space, rows_capacity)
         self.reload(problem, space)
         self.upload()
@@ -72,7 +79,7 @@ class DeviceProblem:
         off = host_bytes = 0
         self._off = {}
         for name in _ARENA_ORDER:
-            need = max(self._need(flat, space, name), 16)
+            need = max(self._need(flat, space, name), self._reserve.get(name, 0), 16)
             cap = _align(need + need // 4 if name in ('rows', 'blocks', 'comp_recs', 'comp_pool') else need)
             if name == 'rows':
                 cap = max(cap, _align(rows_capacity))
@@ -196,6 +203,16 @@ class HetSearcher:
                 self.workspace = torch.empty(need + need // 8, dtype=torch.uint8, device=dp.device)
         if self.want_records and self.records is None:
             self._alloc(self._fixed_capacity if self._fixed_capacity is not None else min(self.shard_plans + 4096, 1 << 18))
+
+    def reserve_workspace(self, num_plans: int) -> None:
+        """Size the workspace for a space of ``num_plans`` plans now, so that rebind() for a smaller one keeps it."""
+        dp = self.dp
+        tile, world = self.shard.tile, self.shard.world
+        need = dp.workspace_bytes(-(-num_plans // (tile * world)) * tile)
+        if self.workspace is None or self.workspace.numel() < need:
+            self.workspace = None
+            with torch.cuda.device(dp.device):
+                self.workspace = torch.empty(need + need // 8, dtype=torch.uint8, device=dp.device)
 
     def _alloc(self, capacity: int) -> None:
         dev = self.dp.device
@@ -397,6 +414,10 @@ class Candidates:
     def __len__(self) -> int:
         return len(self.records)
 
+    def index_of(self, ordinal: int, step: int) -> Optional[int]:
+        """Position of the candidate (ordinal, step), or None: bisection over the (ordinal, step)-sorted records."""
+        return _bisect_records(self.records, 0, len(self.records), int(ordinal), int(step))
+
     def detail_rows(self, idx: np.ndarray) -> np.ndarray:
         if self._detail is None:
             if self._detail_dev is None:
@@ -436,6 +457,260 @@ def materialize(records: np.ndarray, detail: np.ndarray, space: flatten.FlatPlan
     """Records -> the reference's 7-tuples (cost_het_cluster.py:44-46), all of them, eagerly."""
     cand = Candidates(records, detail, space, node_sequences)
     return cand.tuples(np.arange(len(records)))
+
+
+def _bisect_records(rec: np.ndarray, lo: int, hi: int, ordinal: int, step: int) -> Optional[int]:
+    """Index of (ordinal, step) in rec[lo:hi], sorted by (ordinal, step); None when absent."""
+    want = (ordinal, step)
+    end = hi
+    while lo < hi:
+        mid = (lo + hi) >> 1
+        r = rec[mid]
+        if (int(r['ordinal']), int(r['step'])) < want:
+            lo = mid + 1
+        else:
+            hi = mid
+    if lo < end and (int(rec[lo]['ordinal']), int(rec[lo]['step'])) == want:
+        return lo
+    return None
+
+
+# ---------------------------------------------------------------------------------------------
+# windowed search: a space larger than one search holds, walked in ordinal windows (flatten.plan_windows)
+# ---------------------------------------------------------------------------------------------
+_NO_FATAL = 2 ** 64 - 1
+_SUMMED_KEYS = ('num_records', 'num_partition_calls', 'num_balancer_runs', 'num_keyerror', 'num_admitted',
+                'num_chained')
+
+
+@dataclass
+class WindowedOutput:
+    """The merged outputs of the windows searched: ``records`` (host) are every window's records in window order, each
+    window's in (ordinal, step) order - together estimate_costs order; a record of window w has the global ordinal
+    ``bases[w] + ordinal``.  ``firsts[w]`` is the index of window w's first record (``firsts[-1]`` = all records)."""
+    summary: Dict[str, int]
+    best: Optional[Tuple[float, int, int, int, int]]      # cost, GLOBAL ordinal, step, num_repartition, num_stage
+    records: np.ndarray
+    bases: np.ndarray                                     # int64 per window searched
+    firsts: np.ndarray                                    # int64, one more than windows searched
+
+
+class WindowMerge:
+    """Host merge of per-window outputs: counters summed, the best as the lexicographic min of (cost, global ordinal,
+    step), the fatal ordinal made global.  ``add`` returns True at the first window that reports a fatal plan: the
+    reference dies at that plan (quirk Q8), so later windows are not searched."""
+
+    def __init__(self, num_windows: int):
+        self.summary: Dict[str, object] = {k: 0 for k in _SUMMED_KEYS}
+        self.summary.update(fatal_ordinal=_NO_FATAL, fatal_code=0, fatal_aux=0, num_windows=num_windows,
+                            windows_searched=0, instantiation=[])
+        self.best = None
+        self._records: List[np.ndarray] = []
+        self.bases: List[int] = []
+        self.firsts: List[int] = [0]
+
+    def add(self, base: int, summary: Dict[str, int], best, records: Optional[np.ndarray]) -> bool:
+        for k in _SUMMED_KEYS:
+            self.summary[k] += int(summary.get(k, 0))
+        self.summary['windows_searched'] += 1
+        if 'instantiation' in summary:
+            self.summary['instantiation'].append(summary['instantiation'])
+        if best is not None:
+            cand = (best[0], base + int(best[1]), int(best[2]), int(best[3]), int(best[4]))
+            if self.best is None or cand[:3] < self.best[:3]:
+                self.best = cand
+        n = 0 if records is None else len(records)
+        if n:
+            self._records.append(records)
+        self.bases.append(int(base))
+        self.firsts.append(self.firsts[-1] + n)
+        if int(summary.get('fatal_ordinal', _NO_FATAL)) != _NO_FATAL:
+            self.summary.update(fatal_ordinal=base + int(summary['fatal_ordinal']), fatal_code=int(summary['fatal_code']),
+                                fatal_aux=int(summary['fatal_aux']))
+            return True
+        return False
+
+    def result(self) -> WindowedOutput:
+        rec = np.concatenate(self._records) if self._records else np.zeros(0, dtype=native.RECORD_DTYPE)
+        return WindowedOutput(dict(self.summary), self.best, rec, np.asarray(self.bases, dtype=np.int64),
+                              np.asarray(self.firsts, dtype=np.int64))
+
+
+def window_cost_model(problem: flatten.FlatProblem, lib=None) -> Tuple[float, float, float, float]:
+    """(bytes per plan, per byte of rows, per composition record, fixed bytes) of one window's search on the device, from
+    metis_het_workspace_bytes and the buffers the driver allocates around it: the workspace (with HetSearcher's 1/8
+    headroom), a 16 B record slot per plan, and the arena's 1/4 headroom on the rows and composition records."""
+    lib = lib or native.load_library()
+    p = problem.as_struct(lambda n: problem.arrays[n].ctypes.data)
+    n = 1 << 24
+    w1, w2 = (int(lib.metis_het_workspace_bytes(C.byref(p), k, native.METIS_MAX_STAGES)) for k in (n, 2 * n))
+    if min(w1, w2) < 0:
+        native.check(min(w1, w2), 'metis_het_workspace_bytes')
+    per_plan = (w2 - w1) / n * 9 / 8
+    fixed = (w1 - n * (w2 - w1) / n) * 9 / 8 + sum(a.nbytes for a in problem.arrays.values())
+    return per_plan + 16.0, 1.25, 20.0, fixed
+
+
+def window_budget(device, fixed: float) -> float:
+    """Device bytes a window may use: what is free on ``device`` (including memory this process has cached but does not
+    use), less a tenth for the sorts and transfers around a search, less the fixed part of the cost model."""
+    free, _total = torch.cuda.mem_get_info(device)
+    free += torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+    return free * 0.9 - fixed
+
+
+def agree_budget(budget: float, device) -> float:
+    """With torch.distributed initialised: the smallest ``budget`` of all ranks (one all_reduce), so that every rank
+    makes the same one-search / windows choice and cuts the same windows; else ``budget``."""
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return budget
+    t = torch.tensor([int(budget)], dtype=torch.int64, device=device)
+    dist.all_reduce(t, op=dist.ReduceOp.MIN)
+    return float(t.item())
+
+
+def search_windows(problem: flatten.FlatProblem, windows: Sequence[flatten.PlanWindow], device=None, rank: int = 0,
+                   world: int = 1, tile: int = 128) -> Tuple[WindowedOutput, DeviceProblem, 'HetSearcher']:
+    """Search the windows in ordinal order in ONE DeviceProblem arena (sized for every window up front) with ONE
+    HetSearcher (the shard's tiles of every window, workspace sized for the window with the most plans), records only,
+    and merge on the host (WindowMerge).  Afterwards the searcher keeps only what rebuilding candidates needs
+    (metis_het_detail's workspace): the work lists and the record buffer are released."""
+    dp = DeviceProblem(problem, windows[0].space, device, reserve=[w.space for w in windows])
+    searcher = HetSearcher(dp, rank, world, tile, want_records=True, want_detail=False)
+    searcher.reserve_workspace(max(w.space.num_plans for w in windows))
+    merge = WindowMerge(len(windows))
+    for w in windows:
+        if dp.space is not w.space:                           # the first window was uploaded by the constructor
+            dp.reload(problem, w.space)
+            dp.upload()
+            searcher.rebind()
+        out = searcher.run()
+        if merge.add(w.base, out.summary, out.best, np.array(out.records) if out.records is not None else None):
+            break
+    searcher.records = searcher.workspace = None
+    searcher.capacity = 0
+    with torch.cuda.device(dp.device):
+        searcher.workspace = torch.empty(dp.workspace_bytes(0), dtype=torch.uint8, device=dp.device)
+    return merge.result(), dp, searcher
+
+
+def merge_rank_windows(all_counts: np.ndarray, rank_records: Sequence[np.ndarray]) -> Tuple[np.ndarray, np.ndarray]:
+    """The records of every rank -> one list in estimate_costs order.  ``all_counts[r, w]``: records of rank r in
+    window w; ``rank_records[r]``: rank r's records, window by window.  Returns (records, first record per window +
+    total): each window's union ordered by (ordinal, step), windows in order."""
+    world, nwin = all_counts.shape
+    starts = np.concatenate([np.zeros((world, 1), dtype=np.int64), np.cumsum(all_counts, axis=1)], axis=1)
+    parts, firsts = [], [0]
+    for w in range(nwin):
+        union = np.concatenate([rank_records[r][starts[r, w]:starts[r, w + 1]] for r in range(world)])
+        parts.append(union[np.lexsort((union['step'], union['ordinal']))])
+        firsts.append(firsts[-1] + len(union))
+    rec = np.concatenate(parts) if parts else np.zeros(0, dtype=native.RECORD_DTYPE)
+    return rec, np.asarray(firsts, dtype=np.int64)
+
+
+def gather_window_records(merged: WindowedOutput, device) -> WindowedOutput:
+    """Multi-GPU: every rank receives every rank's records, window by window in estimate_costs order (records only).
+    Two all_gathers on ``device``: the per-window record counts and the padded records; then merge_rank_windows.
+    Every rank must have searched the same windows (no fatal plan: api.cost_het_cluster raises before gathering)."""
+    import torch.distributed as dist
+    world = dist.get_world_size()
+    counts = torch.tensor(np.diff(merged.firsts), dtype=torch.int64, device=device)
+    all_counts = _gather_rows(counts).numpy().astype(np.int64)     # [world, windows]
+    cap = max(int(all_counts.sum(axis=1).max()), 1)
+    mine = torch.zeros(cap * 2, dtype=torch.int64, device=device)
+    n_local = len(merged.records)
+    if n_local:
+        mine[:2 * n_local] = torch.from_numpy(np.ascontiguousarray(merged.records).view(np.int64).reshape(-1)).to(device)
+    got = torch.empty(world * cap * 2, dtype=torch.int64, device=device)
+    dist.all_gather_into_tensor(got, mine)
+    flat = got.cpu().numpy().view(native.RECORD_DTYPE).reshape(world, cap)
+    rec, firsts = merge_rank_windows(all_counts, [flat[r] for r in range(world)])
+    return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts)
+
+
+def make_window_ranker(searcher: 'HetSearcher', records: np.ndarray, summary: Dict):
+    """() -> permutation of ``sorted(records, key=cost)`` (stable) for the concatenated records of a windowed search:
+    metis_sort_records(METIS_SORT_BY_COST_STABLE) on the device when the records and the sort workspace fit in free
+    device memory, else numpy's stable sort on the host.  ``summary['ranking']`` says which one ran."""
+    n = len(records)
+    if n > 0xFFFFFFFF:
+        raise NotImplementedError(f'ranking {n} candidates: the rank permutation holds 2^32 indices')
+    dev = searcher.dp.device
+
+    def rank() -> np.ndarray:
+        need = n * 16 + n * 4 + int(searcher.dp.lib.metis_sort_workspace_bytes(C.c_int64(n)))
+        if need <= window_budget(dev, 0.0):
+            with torch.cuda.device(dev):
+                buf = torch.from_numpy(records.view(np.int64).reshape(-1)).to(dev)
+                s = torch.cuda.current_stream(dev)
+                perm = searcher.sort_records(n, native.SORT_BY_COST_STABLE, s, want_perm=True, buf=buf)
+                s.synchronize()
+                out = perm.cpu().numpy().view(np.uint32)
+            summary['ranking'] = 'device'
+            return out
+        summary['ranking'] = 'host'
+        return np.argsort(records['cost'], kind='stable').astype(np.uint32)
+    return rank
+
+
+class WindowedCandidates:
+    """Candidates of a windowed search: only the 16 B records stay on the host.  Device groups, strategies and
+    partitions are rebuilt per request, window by window: the window's rows are regenerated on the device (row kernel)
+    and its picks replayed by metis_het_detail.  The DeviceProblem / HetSearcher of the search are reused (the arena,
+    sized for the largest window's rows, and metis_het_detail's small workspace stay allocated while the result is
+    alive); a window is reloaded whenever the arena holds something else."""
+
+    def __init__(self, records: np.ndarray, bases: np.ndarray, firsts: np.ndarray,
+                 windows: Sequence[flatten.PlanWindow], problem: flatten.FlatProblem, node_sequences: Sequence[Tuple],
+                 searcher: 'HetSearcher'):
+        self.records = records
+        self.cost = records['cost']
+        self.bases = bases
+        self.firsts = firsts
+        self.windows = list(windows)
+        self.problem = problem
+        self.node_sequences = [tuple(s) for s in node_sequences]
+        self.searcher = searcher
+
+    def __len__(self) -> int:
+        return len(self.records)
+
+    def index_of(self, ordinal: int, step: int) -> Optional[int]:
+        """(GLOBAL ordinal, step) -> position, through the window that holds the ordinal."""
+        w = int(np.searchsorted(self.bases, ordinal, side='right')) - 1
+        if w < 0 or w >= len(self.bases):
+            return None
+        rel = int(ordinal) - int(self.bases[w])
+        if rel > 0xFFFFFFFF:
+            return None
+        return _bisect_records(self.records, int(self.firsts[w]), int(self.firsts[w + 1]), rel, int(step))
+
+    def _load(self, w: int) -> DeviceProblem:
+        dp = self.searcher.dp
+        space = self.windows[w].space
+        if dp.space is not space or dp.problem is not self.problem:
+            dp.reload(self.problem, space)                    # metis_het_detail needs no more workspace than it has
+            dp.upload()
+        return dp
+
+    def tuples(self, idx) -> List[Tuple]:
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        if not len(idx):
+            return []
+        win = np.searchsorted(self.firsts, idx, side='right') - 1
+        out: List[Optional[Tuple]] = [None] * len(idx)
+        for w in np.unique(win).tolist():
+            at = np.nonzero(win == w)[0]
+            rec = self.records[idx[at]]
+            dp = self._load(w)
+            detail = self.searcher.detail_for(rec)
+            cand = Candidates(rec, detail, dp.space, self.node_sequences, rows_dev=dp.rows_device())
+            cand._BULK = 1 << 62                              # gather the rows needed, never the whole blob
+            for k, t in zip(at.tolist(), cand.tuples(np.arange(len(rec)))):
+                out[k] = t
+        return out
 
 
 # ---------------------------------------------------------------------------------------------

@@ -30,7 +30,9 @@ DEFAULT_POINTS = [(8, 1, 1, 4), (16, 2, 1, 4), (32, 2, 1, 4), (32, 4, 1, 4), (64
                   (64, 1, 0, 4), (128, 1, 1, 4), (128, 3, 1, 4), (128, 1, 1, 6), (256, 1, 1, 4), (256, 2, 1, 4),
                   (512, 1, 1, 4), (512, 4, 1, 6),
                   # variance 0 (the variance-1 filter collapses the space at >= 256 GPUs, SURVEY.md 8d)
-                  (128, 1, 0, 4), (128, 2, 0, 4), (256, 1, 0, 4)]
+                  (128, 1, 0, 4), (128, 2, 0, 4), (256, 1, 0, 4),
+                  # beyond one search (2^32 plans / 4 GiB of rows / the device's memory): searched in windows
+                  (256, 1, 0, 6), (512, 1, 0, 4), (256, 4, 0, 4)]
 
 
 def run_point(ndev, ntypes, variance, mpl, check):
@@ -47,9 +49,17 @@ def run_point(ndev, ntypes, variance, mpl, check):
     t0 = time.perf_counter()
     problem = flatten.build_problem(profile, cluster, cfg, w.gbs, w.max_tp, w.max_bs, seqs)
     # the host lists the compositions; the GPU writes the rows (SURVEY.md 8(f)-1)
-    space = flatten.build_plan_space(len(seqs), cluster.get_total_num_devices(), w.gbs, w.num_layers, w.variance,
-                                     w.max_permute_len, device_rows=True)
+    space = flatten.build_device_plan_space(len(seqs), cluster.get_total_num_devices(), w.gbs, w.num_layers,
+                                            w.variance, w.max_permute_len)
+    if space is None:                                         # compositions beyond the row kernel: host rows
+        space = flatten.build_plan_space(len(seqs), cluster.get_total_num_devices(), w.gbs, w.num_layers, w.variance,
+                                         w.max_permute_len, device_rows=True)
     enum_ms = 1e3 * (time.perf_counter() - t0)
+    per_plan, per_row, per_rec, fixed = search.window_cost_model(problem)
+    budget = search.window_budget('cuda:0', fixed)
+    if not flatten.fits_one_search(space) or flatten.window_bytes(space, per_plan, per_row, per_rec) > budget:
+        return run_windows(w, tmp, order, seqs, problem, space, flatten.plan_windows(space, budget, per_plan, per_row,
+                                                                                       per_rec), enum_ms, check)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
     dp = search.DeviceProblem(problem, space, 'cuda:0')
@@ -72,11 +82,6 @@ def run_point(ndev, ntypes, variance, mpl, check):
            'host_enumeration_ms': enum_ms, 'gpu_search_ms': ms, 'plans_per_s': space.num_plans / (ms * 1e-3),
            'best': out.best[:3] if out.best else None}
     if check > 0 and space.num_plans:
-        from oracle import metis_oracle as orc
-        ocl = orc.OracleCluster(tmp + '/hostfile', tmp + '/clusterfile.json')
-        oprof, _ = orc.load_profile_dir(tmp + '/profile', order)
-        omodel = orc.OracleModel(w.num_layers, w.hidden_size, w.sequence_length, w.vocab_size, oprof['model']['parameters'])
-        norm = orc.norm_layer_duration(oprof)
         rng = random.Random(ndev * 131 + ntypes)
         limit = out.summary['fatal_ordinal'] if out.summary['fatal_ordinal'] != 2 ** 64 - 1 else space.num_plans
         picks = sorted(rng.sample(range(limit), min(check, limit))) if limit else []
@@ -85,20 +90,84 @@ def run_point(ndev, ntypes, variance, mpl, check):
         by_ord = {}
         for rec, tup in zip(sub, got):
             by_ord.setdefault(int(rec['ordinal']), []).append(tup)
-        bad = 0
-        for o in picks:
-            ns, label, rowi, batches, codes = space.locate(o)
-            plan = {'ns_idx': ns, 'node_sequence': seqs[ns], 'dg_idx': rowi, 'device_groups': [1 << int(c) for c in codes],
-                    'num_stage': label, 'batches': batches, 'gbs': w.gbs}
-            want, counters = [], {'A': 0, 'B': 0, 'C': 0, 'runs': 0, 'keyerr': 0}
-            orc.het_evaluate_plan(oprof, ocl, omodel, norm, plan, o, w.num_layers, w.max_tp, w.max_bs, counters, want)
-            mine = by_ord.get(o, [])
-            same = len(mine) == len(want) and all(
-                (m[1], m[2], m[3], m[4], m[5]) == (x[3], x[4], x[5], x[6], x[7]) and m[6] == x[8] for m, x in zip(mine, want))
-            bad += 0 if same else 1
         row['oracle_checked_plans'] = len(picks)
-        row['oracle_mismatches'] = bad
+        row['oracle_mismatches'] = oracle_mismatches(w, tmp, order, seqs, picks, space.locate,
+                                                     lambda o: by_ord.get(o, []))
     return row
+
+
+def run_windows(w, tmp, order, seqs, problem, space, windows, enum_ms, check):
+    """A point beyond one search: the windows of flatten.plan_windows searched in ordinal order (search.search_windows).
+    The time is the wall time of search.search_windows (every window's upload, row generation and search, and the host
+    merges), host enumeration excluded.  The parity check takes each picked plan from the windows (PlanWindow.plan_at)
+    and its device groups from the host enumerator's table of its stage count."""
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()                                  # the peak below is this point's alone
+    torch.cuda.reset_peak_memory_stats()
+    t1 = time.perf_counter()
+    merged, dp, searcher = search.search_windows(problem, windows, 'cuda:0')
+    torch.cuda.synchronize()
+    ms = 1e3 * (time.perf_counter() - t1)
+    s = merged.summary
+    row = {'ndev': w_ndev(w), 'types': len(w.device_types()), 'variance': w.variance, 'mpl': w.max_permute_len,
+           'layers': w.num_layers, 'gbs': w.gbs, 'A_plans': space.num_plans, 'row_bytes': int(space.rows_total_bytes),
+           'windows': len(windows), 'windows_searched': s['windows_searched'],
+           'B_partition_calls': s['num_partition_calls'], 'runs': s['num_balancer_runs'], 'C_costed': s['num_records'],
+           'keyerror': s['num_keyerror'], 'fatal_ordinal': None if s['fatal_ordinal'] == 2 ** 64 - 1 else s['fatal_ordinal'],
+           'host_enumeration_ms': enum_ms, 'gpu_search_ms': ms, 'plans_per_s': space.num_plans / (ms * 1e-3),
+           'peak_device_bytes': int(torch.cuda.max_memory_reserved()), 'best': merged.best[:3] if merged.best else None}
+    if check > 0 and space.num_plans:
+        cand = search.WindowedCandidates(merged.records, merged.bases, merged.firsts, windows, problem, seqs, searcher)
+        rng = random.Random(w_ndev(w) * 131 + len(w.device_types()))
+        limit = row['fatal_ordinal'] if row['fatal_ordinal'] is not None else space.num_plans
+        picks = sorted(rng.sample(range(limit), min(check, limit))) if limit else []
+        picks = sorted(set(picks) | {o for x in windows for o in (x.base, x.base + x.space.num_plans - 1) if o < limit})
+        rec = merged.records
+        glob = merged.bases[np.searchsorted(merged.firsts, np.arange(len(rec)), side='right') - 1] + \
+            rec['ordinal'].astype(np.int64)
+        bases = np.asarray([x.base for x in windows], dtype=np.int64)
+        table = {}
+
+        def plan_of(o):
+            # the device groups from the host enumerator's table of the stage count, not from the windows' rows
+            ns, label, dg, batches, S, _at = windows[int(np.searchsorted(bases, o, side='right')) - 1].plan_at(o)
+            if S not in table:
+                table.clear()
+                table[S] = flatten.enumerate_device_groups(S, w_ndev(w), w.variance, w.max_permute_len)
+            return ns, label, dg, batches, table[S][dg]
+
+        def mine_of(o):
+            idx = np.nonzero(glob == o)[0]
+            return cand.tuples(idx) if len(idx) else []
+        row['oracle_checked_plans'] = len(picks)
+        row['oracle_mismatches'] = oracle_mismatches(w, tmp, order, seqs, picks, plan_of, mine_of)
+    return row
+
+
+def oracle_mismatches(w, tmp, order, seqs, picks, plan_of, mine_of) -> int:
+    """Plans of ``picks`` whose candidates (``mine_of(ordinal)``: the GPU's 7-tuples) differ from the pinned oracle's;
+    ``plan_of(ordinal)`` -> (ns_idx, label, dg_idx, batches, log2 device groups)."""
+    from oracle import metis_oracle as orc
+    ocl = orc.OracleCluster(tmp + '/hostfile', tmp + '/clusterfile.json')
+    oprof, _ = orc.load_profile_dir(tmp + '/profile', order)
+    omodel = orc.OracleModel(w.num_layers, w.hidden_size, w.sequence_length, w.vocab_size, oprof['model']['parameters'])
+    norm = orc.norm_layer_duration(oprof)
+    bad = 0
+    for o in picks:
+        ns, label, rowi, batches, codes = plan_of(o)
+        plan = {'ns_idx': ns, 'node_sequence': seqs[ns], 'dg_idx': rowi, 'device_groups': [1 << int(c) for c in codes],
+                'num_stage': label, 'batches': batches, 'gbs': w.gbs}
+        want, counters = [], {'A': 0, 'B': 0, 'C': 0, 'runs': 0, 'keyerr': 0}
+        orc.het_evaluate_plan(oprof, ocl, omodel, norm, plan, o, w.num_layers, w.max_tp, w.max_bs, counters, want)
+        mine = mine_of(o)
+        same = len(mine) == len(want) and all(
+            (m[1], m[2], m[3], m[4], m[5]) == (x[3], x[4], x[5], x[6], x[7]) and m[6] == x[8] for m, x in zip(mine, want))
+        bad += 0 if same else 1
+    return bad
+
+
+def w_ndev(w):
+    return sum(n for _, n in w.nodes)
 
 
 def main():
