@@ -70,6 +70,7 @@ struct OneLane {
         return lo;
     }
     MB_HD int bcast_last(int v) const { return v; }
+    MB_HD static void assume_shared(const void *) {}
     MB_HD void argmax_first(double &, int &) const {}
     MB_HD void argmin_first(double &, int &) const {}
     MB_HD void imax_first(int &, int &) const {}
@@ -315,9 +316,13 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     MB_HD CoopEvaluator(const Tables &t, Scratch<MAXS, MAXL> &s, CoopMail &mb, const X &lanes)
         : Base(t, s), x(lanes), mail(mb) {}
 
+    // start of every phase: the scratch and the mailbox are the warp's shared memory (X::assume_shared)
+    MB_HD void shared_scratch() const { X::assume_shared(&w); X::assume_shared(&mail); }
+
     // Start of a plan: groups, rank starts and the first strategy that can be valid (PlanEvaluator::begin,
     // search_space/plan.py:231-249).  The admission pass already dropped plans whose first strategy is invalid.
     MB_HD void begin_coop(const PlanDesc &plan) {
+        shared_scratch();
         pd = plan;
         bs_total = T.p.gbs / pd.batches;
         int lb = 0;
@@ -346,6 +351,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // IntraStagePlanGenerator._next_strategy (search_space/plan.py:251-268): the stage with the smallest memory
     // state (or, without a state, the largest dp) that still has dp != 1 halves its dp; first one among equals.
     MB_HD bool next_strategy_coop(bool have_state) {
+        shared_scratch();
         int pick = 0x7FFFFFFF;
         if (have_state) {
             double best = INFINITY;
@@ -376,6 +382,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
 
     // first stage (in stage order) whose error mailbox is set: leader scan, rare path
     MB_HD_NOINLINE int first_error(const double *box, int n) {
+        shared_scratch();
         x.sync();
         if (x.leader()) {
             mail.err = 0;
@@ -395,6 +402,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
 
     // StagePerformance.get_intra_stage_compute_performance (model/device_group.py:54-85) -> w.perf
     MB_HD int compute_performance_coop() {
+        shared_scratch();
         bool failed = false;
         x.sync();
         METIS_PAR(x, s, pd.S) {
@@ -428,6 +436,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // (induction over the stages).  If any stage fails (a compare decided by the last bits), the leader runs the
     // sequential pass.  returns true when the forward state (w.fe, w.capa, mail.k / s_top / top_skip) is final.
     MB_HD bool forward_coop() {
+        shared_scratch();
         const int S = pd.S, last = S - 1;
         const int L = T.p.num_layers;
         if (S < 4 || T.p.norm_len < L) { x.note(kPathSeqForward); return false; }   // nothing to overlap: sequential pass
@@ -500,6 +509,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     //               whole warp per sub-layer.
     // Writes w.capa, w.fe, w.lstk, the middle block's stages (bytes of w.subw), mail.k / m.  returns METIS_FATAL_* (0 = ok)
     MB_HD int fill_coop() {
+        shared_scratch();
         const int S = pd.S, last = S - 1;
         const double *dlay = T.dlay;
         x.sync();
@@ -610,6 +620,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
 
     // LayerComputeBalancer.run (model/load_balancer.py:197-207): w.perf -> w.part, w.cnt
     MB_HD int balance_coop() {
+        shared_scratch();
         const int S = pd.S;
         const int L = T.p.num_layers;
         if (T.p.norm_len < L) return METIS_FATAL_INDEX;       // expand_lc_demand[layer_id] IndexError (:219/:238)
@@ -623,48 +634,52 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         if (rc_tail) return rc_tail;
         const int m = mail.m;
         x.gate(kGateVote, 13);
-        // ---- majority vote back to real layers (:290-308), one layer per lane ----
+        // ---- majority vote back to real layers (:290-308), a block of ceil(L / 32) consecutive layers per lane ----
         // Stage of sub-layer j, from the interval ends: j >= m -> last stage (backward tail); k <= j < m -> where
         // the middle block put it (bytes of subw); below k the forward slot t = #{u : start of stage u+1 <= j}, and if j is
         // that slot's skipped sub-layer: last stage when the backward pass took it, else where it was placed (lstk).
+        // The slot is searched for once, at the block's first sub-layer; from there it only moves up.
         const int kfwd = mail.k;
-        METIS_PAR(x, r, L) {
-            const int j0 = kH * r;
-            int own = kDropped;
-            if (j0 >= m) {
-                own = last;
-            } else {
-                int t = 0;
-                if (j0 < kfwd) {                             // first slot whose successor starts above j0
-                    int lo = 0, hi = last - 1;               // (j0 < k: such a slot exists among 0 .. last-1)
+        const int B = (L + 31) >> 5;                          // layers per block; trailing blocks may be empty
+        METIS_PAR(x, blk, 32) {
+            const int r0 = blk * B, r1 = r0 + B < L ? r0 + B : L;
+            const int j0 = kH * r0;
+            int t = 0;
+            if (j0 < kfwd && j0 < m) {                       // first slot whose successor starts above j0
+                int lo = 0, hi = last - 1;                   // (j0 < k: such a slot exists among 0 .. last-1)
 #pragma unroll 1
-                    while (lo < hi) {
-                        const int mid = (lo + hi) >> 1;
-                        const uint16_t e = w.fe[mid];
-                        if ((int)(e & kPos) + ((e & kBroke) ? 1 : 0) <= j0) lo = mid + 1; else hi = mid;
-                    }
-                    t = lo;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    const uint16_t e = w.fe[mid];
+                    if ((int)(e & kPos) + ((e & kBroke) ? 1 : 0) <= j0) lo = mid + 1; else hi = mid;
                 }
-                uint64_t v = 0xFF00000000000000ULL;
-                uint16_t e = w.fe[t];                        // slot t: its end, and where stage t + 1 starts
-                int nxt = (int)(e & kPos) + ((e & kBroke) ? 1 : 0);
-#pragma unroll 1
-                for (int q = 0; q < kH; ++q) {
-                    const int j = j0 + q;
-                    int st;
-                    if (j >= m) st = last;
-                    else if (j >= kfwd) st = reinterpret_cast<const uint8_t *>(w.subw)[j - kfwd];
-                    else {
-#pragma unroll 1
-                        while (nxt <= j) { ++t; e = w.fe[t]; nxt = (int)(e & kPos) + ((e & kBroke) ? 1 : 0); }
-                        st = t;
-                        if (nxt - 1 == j && (e & kBroke)) st = (e & kTaken) ? last : (int)w.lstk[t];
-                    }
-                    v |= (uint64_t)st << (8 * q);
-                }
-                own = layer_owner(v, (T.p.corrected & METIS_FIX_Q5) != 0);
+                t = lo;
             }
-            reinterpret_cast<uint8_t *>(w.ownerw)[r] = (uint8_t)own;
+            uint16_t e = w.fe[t];                            // slot t: its end, and where stage t + 1 starts
+            int nxt = (int)(e & kPos) + ((e & kBroke) ? 1 : 0);
+#pragma unroll 1
+            for (int r = r0; r < r1; ++r) {
+                int own = last;
+                if (kH * r < m) {
+                    uint64_t v = 0xFF00000000000000ULL;
+#pragma unroll 1
+                    for (int q = 0; q < kH; ++q) {
+                        const int j = kH * r + q;
+                        int st;
+                        if (j >= m) st = last;
+                        else if (j >= kfwd) st = reinterpret_cast<const uint8_t *>(w.subw)[j - kfwd];
+                        else {
+#pragma unroll 1
+                            while (nxt <= j) { ++t; e = w.fe[t]; nxt = (int)(e & kPos) + ((e & kBroke) ? 1 : 0); }
+                            st = t;
+                            if (nxt - 1 == j && (e & kBroke)) st = (e & kTaken) ? last : (int)w.lstk[t];
+                        }
+                        v |= (uint64_t)st << (8 * q);
+                    }
+                    own = layer_owner(v, (T.p.corrected & METIS_FIX_Q5) != 0);
+                }
+                reinterpret_cast<uint8_t *>(w.ownerw)[r] = (uint8_t)own;
+            }
         }
         METIS_PAR(x, s, S) w.cnt[s] = 0;
         x.sync();
@@ -754,6 +769,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // LayerLoadBalancer._adj_compute_performance (model/load_balancer.py:71-107)
     // in: w.perf (c_capa), w.extra (m_demand); out: w.perf; returns 1 = None, 0 ok, <0 fatal (negated code)
     MB_HD int adjust_performance_coop() {
+        shared_scratch();
         const int S = pd.S;
         double *ratio = reinterpret_cast<double *>(w.subw);      // free after the vote (MAXL >= MAXS)
         x.sync();
@@ -811,6 +827,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // One attempt of LayerLoadBalancer.partition_layer after the balancer (model/load_balancer.py:127-143):
     // memory demand (:29-55), OOM test (:57-63), capacity re-weighting.  Returns like PlanEvaluator::memory_phase.
     MB_HD int memory_phase_coop(int attempt) {
+        shared_scratch();
         const int S = pd.S;
         bool failed = false, oom = false;
         x.sync();                                            // the balancer's last readers of capa / extra / mstate are done
@@ -842,6 +859,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     // HeteroCostEstimator.get_cost (model/cost_estimator.py:199-244); returns 0 ok, 1 KeyError.  The cost lands in
     // mail.val (every lane reads it after the final sync).
     MB_HD int get_cost_coop(double &cost_out) {
+        shared_scratch();
         const bool one_type = ONE || T.p.num_types == 1;
         const int nstage = pd.label < pd.S ? pd.label : pd.S;  // zip(range(plan.num_stage), strategies)
         // rank_node_map holds num_nodes * devices(node 0) ranks (cluster_bandwidth.py:34-47, Q10): beyond -> KeyError

@@ -125,6 +125,11 @@ struct WarpCoop {
         return n + 1;
     }
     __device__ int bcast_last(int v) const { return __shfl_sync(0xFFFFFFFFu, v, 31); }
+    // A CoopEvaluator on this policy keeps its scratch and mailbox in shared memory (het_chain_kernel, tests/devsim);
+    // every phase says so (CoopEvaluator::shared_scratch).  The compiler does not infer it through the evaluator's
+    // references, and generic 64-bit addressing costs the issue-bound chain kernel instructions and registers at
+    // every access.
+    static __device__ void assume_shared(const void *p) { __builtin_assume(__isShared(p)); }
     // Reductions with REDUX (one instruction per 32-bit max / min over the warp) on an order-preserving integer
     // image of the double (-0.0 and +0.0 share one key, like ==); no NaN reaches these.
     static __device__ __forceinline__ unsigned long long dkey(double v) {
