@@ -42,6 +42,13 @@ class Workload:
     memory_gb: Dict[str, float] = field(default_factory=dict)   # override per type
     intra_bw: Dict[str, float] = field(default_factory=dict)    # override per type
     profile_layers: int = 0                      # 0 -> num_layers
+    # 'default': one layer shape for every key, scaled by type, tp and bs (the BASELINE configs);
+    # 'rough': per-type shapes, per-key noise and memory, planted ties (see _rough_profiles)
+    profile_style: str = 'default'
+    int_memory: Sequence[str] = ()               # rough: types whose memory lists are all-int
+    short_memory: bool = False                   # rough: memory lists one entry shorter than the compute lists
+    zero_fb_sync: Sequence[Tuple[str, int, int]] = ()   # rough: keys with forward_backward == sum(layer computes)
+    missing: Sequence[Tuple[str, int, int]] = ()        # rough: keys left unprofiled
 
     def device_types(self) -> List[str]:
         seen: List[str] = []
@@ -83,17 +90,99 @@ def _profile_json(dev: str, tp: int, bs: int, base: List[float], num_layers: int
     }
 
 
+def _rough_shape(rng: random.Random, n: int, first, mid, last) -> Tuple[List[float], List[bool]]:
+    """n per-layer values: first(), mid() for the middle layers with runs of equal values, last();
+    ``same[j]`` marks a layer that repeats layer j - 1."""
+    vals, same = [first()], [False]
+    for _ in range(n - 2):
+        if len(vals) > 1 and rng.random() < 0.2:
+            vals.append(vals[-1])
+            same.append(True)
+        else:
+            vals.append(mid())
+            same.append(False)
+    return vals + [last()], same + [False]
+
+
+def _rough_profiles(w: Workload, nl: int, rng: random.Random) -> Dict[Tuple[str, int, int], dict]:
+    """Profiles whose values differ by device type, key and layer (profile_style='rough').
+
+    Per type: a compute shape log-uniform over three decades with embedding-like first and last layers, and a memory
+    shape of its own.  Per key: compute and memory rows with multiplicative noise (rows of one type are not
+    proportional across tp and bs), runs of equal layers kept, forward_backward_time_ms a little above or below the
+    layers' sum, or equal to it for the keys in ``w.zero_fb_sync`` (fb_sync == 0.0).  Memory lists are all-int for
+    ``w.int_memory`` and all-float otherwise.  The second type repeats the first type's compute row bit for bit at one
+    key.  Keys in ``w.missing`` are not written."""
+    from .flatten import py312_sum                  # the builtin sum of CPython >= 3.12, the reference's own
+    types = w.device_types()
+    tie_key = (w.tps[len(w.tps) // 2], w.bss[len(w.bss) // 2])
+
+    def log_uniform():                              # 0.05 .. ~63: 10**(k/10) by repeated products, k in [0, 30)
+        x = 0.05
+        for _ in range(rng.randrange(30)):
+            x *= 1.2589254117941673
+        return x * (1 + 0.25 * rng.random())
+
+    out: Dict[Tuple[str, int, int], dict] = {}
+    for ti, dev in enumerate(types):
+        shape, same = _rough_shape(rng, nl, lambda: 0.2 + 0.3 * rng.random(), log_uniform,
+                                   lambda: 3 + 5 * rng.random())
+        mshape, msame = _rough_shape(rng, nl, lambda: 6000 + 4000 * rng.random(), lambda: 1500 + 5000 * rng.random(),
+                                     lambda: 9000 + 6000 * rng.random())
+        speed = SPEED[dev]
+        for tp in w.tps:
+            for bs in w.bss:
+                lc: List[float] = []
+                for j in range(nl):
+                    lc.append(lc[-1] if same[j] else shape[j] * speed * bs * TP_SCALE[tp] * (0.9 + 0.2 * rng.random()))
+                mem: list = []
+                for j in range(nl):
+                    mem.append(mem[-1] if msame[j] else mshape[j] / tp * (1 + 0.1 * bs) * (0.95 + 0.1 * rng.random()))
+                if dev in w.int_memory:
+                    mem = [int(m) for m in mem]
+                if w.short_memory:
+                    mem = mem[:-1]
+                if ti == 1 and (tp, bs) == tie_key:
+                    lc = list(out[(types[0], tp, bs)]['execution_time']['layer_compute_total_ms'])
+                total = py312_sum(lc)
+                r = rng.random()
+                if (dev, tp, bs) in w.zero_fb_sync:
+                    fb = total
+                elif r < 0.3:
+                    fb = total * (1 - 0.002 * (1 + r))
+                else:
+                    fb = total * (1.05 + 0.1 * r)
+                params = [393216000] + [202383360] * (nl - 2) + [393220096]
+                out[(dev, tp, bs)] = {
+                    'model': {'model_name': 'SYN', 'num_layers': nl,
+                              'parameters': {'total_parameters_bytes': sum(params), 'parameters_per_layer_bytes': params}},
+                    'execution_time': {'total_time_ms': 1.4 * total, 'forward_backward_time_ms': fb,
+                                       'batch_generator_time_ms': 0.9, 'layernorm_grads_all_reduce_time_ms': 0.02,
+                                       'embedding_grads_all_reduce_time_ms': 0.04, 'optimizer_time_ms': 40 / tp,
+                                       'layer_compute_total_ms': lc},
+                    'execution_memory': {'total_memory': 0, 'layer_memory_total_mb': mem},
+                }
+    for key in w.missing:
+        del out[tuple(key)]
+    return out
+
+
 def materialize(w: Workload, root: str) -> str:
     """Write w's files under ``root``; returns sha256 over all generated bytes."""
     os.makedirs(os.path.join(root, 'profile'), exist_ok=True)
     rng = random.Random(w.seed)
     nl = w.profile_layers or w.num_layers
-    base = [0.3] + [10 + rng.random() for _ in range(nl - 2)] + [0.4]
+    rough = _rough_profiles(w, nl, rng) if w.profile_style == 'rough' else None
+    if rough is None:
+        base = [0.3] + [10 + rng.random() for _ in range(nl - 2)] + [0.4]
     digest = hashlib.sha256()
     for dev in w.device_types():
         for tp in w.tps:
             for bs in w.bss:
-                text = json.dumps(_profile_json(dev, tp, bs, base, nl), indent=1)
+                if rough is not None and (dev, tp, bs) not in rough:
+                    continue
+                prof = rough[(dev, tp, bs)] if rough is not None else _profile_json(dev, tp, bs, base, nl)
+                text = json.dumps(prof, indent=1)
                 with open(os.path.join(root, 'profile', f'DeviceType.{dev}_tp{tp}_bs{bs}.json'), 'w') as fh:
                     fh.write(text)
                 digest.update(text.encode())
@@ -115,7 +204,8 @@ def materialize(w: Workload, root: str) -> str:
 
 def profile_file_order(w: Workload) -> List[str]:
     """A fixed listing order for the profile directory (pins quirk Q3 in tests/bench)."""
-    return [f'DeviceType.{dev}_tp{tp}_bs{bs}.json' for dev in w.device_types() for tp in w.tps for bs in w.bss]
+    return [f'DeviceType.{dev}_tp{tp}_bs{bs}.json' for dev in w.device_types() for tp in w.tps for bs in w.bss
+            if (dev, tp, bs) not in w.missing]
 
 
 def _nodes(*spec: Tuple[str, int]) -> List[Tuple[str, int]]:
@@ -186,6 +276,40 @@ WORKLOADS: Dict[str, Workload] = {w.name: w for w in [
     Workload('lim_s128_l255', _nodes(('A100', 16)), 255, 8, 4096, 1024, 51200, max_permute_len=1),     # <128,256,1>
     Workload('lim_s128_t2', _nodes(('A100', 8), ('H100', 8)), 129, 2, 4096, 1024, 51200, max_permute_len=1,
              bss=(1, 2, 4, 8), memory_gb={'A100': 58, 'H100': 64}),                                    # <128,256,0> by S
+    # rough profiles (profile_style='rough'): memory that depends on the device type, compute rows that are not one
+    # shape scaled, int memory lists, fb_sync == 0.0 and unprofiled keys, so that which type's / key's table the
+    # search reads changes the result (tests/test_rough_profiles.py)
+    # mixed-type stages and tight memory; the two node sequences start with different types (quirk Q6)
+    Workload('rough_mix2', _nodes(('A100', 1), ('V100', 3)), 12, 32, 1024, 512, 30522, bss=(1, 2, 4, 8, 16),
+             memory_gb={'A100': 40, 'V100': 16}, int_memory=('V100',), seed=101, profile_style='rough'),
+    # three types, all six node sequences, nodes of 4 GPUs
+    Workload('rough_t3', [('A100', 4), ('H100', 4), ('V100', 4), ('V100', 4)], 10, 16, 1024, 512, 30522,
+             bss=(1, 2, 4, 8, 16), memory_gb={'A100': 24, 'H100': 32, 'V100': 16}, int_memory=('H100',), seed=102,
+             profile_style='rough'),
+    # unequal nodes, node 0 largest (quirk Q10 rank lists) with type-dependent memory
+    Workload('rough_q10', [('A100', 8), ('H100', 4), ('V100', 4)], 12, 32, 1024, 512, 30522, bss=(1, 2, 4, 8, 16),
+             memory_gb={'A100': 24, 'H100': 40, 'V100': 16}, seed=103, profile_style='rough'),
+    # 15 profiled layers for 10 model layers, memory lists of 14 int entries
+    Workload('rough_long_int', _nodes(('A100', 1), ('H100', 1)), 10, 32, 1024, 512, 30522, profile_layers=15,
+             memory_gb={'A100': 16, 'H100': 24}, int_memory=('A100', 'H100'), short_memory=True, seed=104,
+             profile_style='rough'),
+    # fb_sync == 0.0 at two keys (per-candidate KeyError, quirk Q9) and a key only one type has
+    Workload('rough_keys', [('A100', 4), ('H100', 4), ('H100', 4), ('H100', 4)], 12, 32, 1024, 512, 30522,
+             bss=(1, 2, 4, 8, 16), memory_gb={'A100': 24, 'H100': 24}, seed=105,
+             zero_fb_sync=(('H100', 2, 2), ('A100', 1, 4)), missing=(('H100', 4, 8),), profile_style='rough'),
+    # the same with a searched key missing for one type: the reference aborts with KeyError at plan 11
+    Workload('rough_keys_fatal', [('A100', 4), ('H100', 4), ('H100', 4), ('H100', 4)], 12, 32, 1024, 512, 30522,
+             bss=(1, 2, 4, 8, 16), memory_gb={'A100': 24, 'H100': 24}, seed=105,
+             zero_fb_sync=(('H100', 2, 2), ('A100', 1, 4)), missing=(('H100', 1, 4),), profile_style='rough'),
+    # max_permute_len 1 in the larger instantiations: <96,128,0> by the stage count, <128,256,0> by the layer count
+    Workload('rough_s66_t2', _nodes(('A100', 8), ('H100', 8)), 66, 8, 4096, 1024, 51200, max_permute_len=1,
+             bss=(1, 2, 4, 8), memory_gb={'A100': 48, 'H100': 40}, seed=106, profile_style='rough'),
+    Workload('rough_l130_t2', _nodes(('A100', 1), ('H100', 1)), 130, 8, 4096, 1024, 51200, max_permute_len=1,
+             bss=(1, 2, 4, 8), memory_gb={'A100': 240, 'H100': 240}, seed=107, profile_style='rough'),
+    # single type for the homogeneous path (cost_homo_cluster): int memory, a zero fb_sync, an unprofiled key
+    Workload('rough_homo', _nodes(('H100', 2)), 20, 64, 4096, 1024, 51200, bss=(1, 2, 4, 8), memory_gb={'H100': 40},
+             zero_fb_sync=(('H100', 2, 1),), missing=(('H100', 4, 8),), int_memory=('H100',), seed=108,
+             profile_style='rough'),
 ]}
 
 
