@@ -308,6 +308,53 @@ int64_t metis_enum_compositions(int32_t first_stage, int32_t last_stage, int32_t
 /* device: recs / pool [device], rows [device] receives every row (same layout as metis_enum_device_group_tables) */
 int metis_generate_rows(const MetisCompRec *recs, int64_t num_comps, const uint8_t *pool, uint8_t *rows, void *stream);
 
+/*
+ * Device-side listing of the compositions (SURVEY.md 8(f)-1): the same compositions, merged groups, row counts and
+ * records as metis_enum_compositions, listed on the GPU one thread per composition (a composition is found from its
+ * rank through a table of completion counts, so nothing walks the list), and handed out window by window: the host
+ * never holds the whole list, only one window's records and pool.
+ *   1. metis_list_workspace_bytes  (host only) sizes the workspace; optionally the compositions of each stage count
+ *   2. metis_list_stages           lists every composition of first_stage..last_stage into the workspace and writes
+ *                                  the rows of each stage count (what rows_per_stage of metis_enum_compositions holds)
+ *   3. metis_list_window           for a set of row ranges, one per (stage count, rows) the window covers, writes the
+ *                                  window's records and pool (call with recs == NULL to size)
+ * A window's rows are its ranges back to back, in the order given: a record's row_offset is relative to that layout,
+ * its pool_offset to the window's own pool.  The records of a range are metis_enum_compositions' slices cut to the
+ * range (first_row = offset of the slice's first row inside the composition).  The workspace of step 2 must be kept,
+ * unchanged, for step 3.
+ */
+typedef struct MetisListing {
+    int32_t first_stage;          /* stage counts first_stage .. last_stage (last_stage <= METIS_MAX_STAGES)      */
+    int32_t last_stage;
+    int32_t num_gpus;
+    int32_t max_permute_len;
+    double variance;              /* --min_group_scale_variance                                                  */
+    int32_t max_ranges;           /* most row ranges of one metis_list_window call                               */
+    int32_t reserved;
+} MetisListing;
+
+typedef struct MetisRowRange {
+    int32_t stages;               /* stage count of the range                                                    */
+    int32_t reserved;
+    int64_t first_row;            /* rows [first_row, end_row) of the stage count's table                        */
+    int64_t end_row;
+} MetisRowRange;
+
+/* host: bytes of device workspace for `listing` (METIS_E_ARG when it cannot be listed); comps_per_stage [host],
+ * optional: last_stage - first_stage + 1 int64, the compositions of each stage count */
+int64_t metis_list_workspace_bytes(const MetisListing *listing, int64_t *comps_per_stage);
+/* rows_per_stage [host] last_stage - first_stage + 1 int64; max_groups [host] the most merged groups of any
+ * composition (a composition above METIS_MAX_PERMUTE_GROUPS is counted but never written as a record) */
+int metis_list_stages(const MetisListing *listing, void *workspace, int64_t workspace_bytes, int64_t *rows_per_stage,
+                      int32_t *max_groups, void *stream);
+/* ranges [host] num_ranges <= listing->max_ranges; recs / pool [device] or NULL; sizes [host] 3 int64: records, pool
+ * bytes, status (0 = written; bit 0: a range outside its stage count's table, bit 1: a composition of more than
+ * METIS_MAX_PERMUTE_GROUPS merged groups in a range (its records are not written), bit 2: recs / pool too small
+ * (nothing written)) */
+int metis_list_window(const MetisListing *listing, void *workspace, int64_t workspace_bytes, const MetisRowRange *ranges,
+                      int32_t num_ranges, MetisCompRec *recs, int64_t recs_capacity, uint8_t *pool,
+                      int64_t pool_capacity, int64_t *sizes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -233,10 +233,13 @@ class HetSearchResult(Sequence):
 
 def het_problem(args, gpu_cluster, profile_data, model_config, layer_load_balancer=None,
                 node_sequences: Optional[Sequence[Sequence]] = None, corrected: Sequence[str] = (),
-                rows_out: Optional[np.ndarray] = None, device_rows: bool = False, unbounded: bool = False):
+                rows_out: Optional[np.ndarray] = None, device_rows: bool = False, unbounded: bool = False,
+                rows_per_stage: Optional[np.ndarray] = None):
     """Flatten the inputs of cost_het_cluster() (order of ``set(device_types)`` = quirk Q4).  ``device_rows``: the
     host lists only the compositions, the GPU writes the device-group rows (SURVEY.md 8(f)-1).  ``unbounded`` (with
-    ``device_rows``): a space beyond the limits of one search is returned too, for a windowed search."""
+    ``device_rows``): a space beyond the limits of one search is returned too, for a windowed search.
+    ``rows_per_stage`` (a device listing's, metis_b200.listing): the space is only its block list
+    (flatten.listed_plan_space); its windows get their records from the listing."""
     if node_sequences is None:
         node_sequences = list(permutations(set(gpu_cluster.get_device_types())))
     norm = layer_load_balancer.norm_layer_duration if layer_load_balancer is not None else None
@@ -244,7 +247,10 @@ def het_problem(args, gpu_cluster, profile_data, model_config, layer_load_balanc
                                     args.max_profiled_tp_degree, args.max_profiled_batch_size, node_sequences,
                                     norm, corrected=corrected)
     space = None
-    if device_rows and unbounded:
+    if rows_per_stage is not None:
+        space = flatten.listed_plan_space(len(node_sequences), gpu_cluster.get_total_num_devices(), args.gbs,
+                                          args.num_layers, rows_per_stage, corrected=corrected)
+    elif device_rows and unbounded:
         space = flatten.build_device_plan_space(len(node_sequences), gpu_cluster.get_total_num_devices(), args.gbs,
                                                 args.num_layers, args.min_group_scale_variance, args.max_permute_len,
                                                 corrected=corrected)
@@ -313,13 +319,24 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     dist = torch.distributed if (torch.distributed.is_available() and torch.distributed.is_initialized()) else None
     rank, world = (dist.get_rank(), dist.get_world_size()) if dist else (0, 1)
     dev = search._require_cuda(device)
-    # the host lists the compositions (a few thousand records); the rows themselves are written by the GPU
+    if node_sequences is None:
+        node_sequences = list(permutations(set(gpu_cluster.get_device_types())))
+    listing = _device_listing(args, gpu_cluster, len(node_sequences), dev)
+    # the host or, for a large space, the GPU lists the compositions; the rows themselves are written by the GPU
     problem, space, seqs = het_problem(args, gpu_cluster, profile_data, model_config, layer_load_balancer,
-                                       node_sequences, corrected=tuple(corrected), device_rows=True, unbounded=True)
+                                       node_sequences, corrected=tuple(corrected), device_rows=True, unbounded=True,
+                                       rows_per_stage=listing.rows_per_stage if listing is not None else None)
+    if listing is None:
+        windows = _het_windows(problem, space, dev, rank, world)
+    else:
+        windows = _listed_windows(problem, space, listing, dev, rank, world)
+        if len(windows) == 1:                                 # one search: the window is the whole space
+            space, windows = windows[0].space, None
     t1 = time.perf_counter()
-    windows = _het_windows(problem, space, dev, rank, world)
     if windows is not None:
-        return _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1)
+        result = _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1)
+        result.summary['listing'] = 'host' if listing is None else 'device'
+        return result
     stride = 3 * int(space.blocks['num_stage'].max()) + 1
     dp, searcher = _engine(problem, space, dev, rank, world, stride)
     dp.upload()
@@ -355,7 +372,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     # sorted(result, key=cost) is the CALLER's step in the reference (cost_het_cluster.py:76): its permutation is
     # computed by the device sort when ranked() is first asked for; best() needs no sort at all
     result = HetSearchResult(cand, out.rank_order,
-                             dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)), num_windows=1),
+                             dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)), num_windows=1,
+                                  listing='host' if listing is None else 'device'),
                              ranker=search.make_ranker(searcher, out.records_dev) if len(out.records) else None,
                              best_key=(best[1], best[2]) if best else None)
     result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
@@ -368,6 +386,42 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
 _ONE_SEARCH_BYTES = 1 << 31
 # Below this budget a windowed search is refused: its windows would be so small that reloading them dominates.
 _MIN_WINDOW_BYTES = 1 << 30
+
+
+# A space of more compositions than this is listed on the GPU (metis_b200.listing): the host then holds one window's
+# composition records at a time instead of the whole space's, and spends milliseconds instead of seconds listing them.
+# Below it the host enumerator lists them (metis_enum_compositions), which is as fast for spaces of this size.
+_DEVICE_LISTING_COMPS = 1 << 18
+
+
+def _device_listing(args, gpu_cluster, num_node_sequences: int, dev):
+    """The device listing of the space of ``args`` when it has more than _DEVICE_LISTING_COMPS compositions, else
+    None (also when a composition has more merged groups than the row kernel handles: the host path decides then)."""
+    from . import listing as listing_mod
+    num_devices = gpu_cluster.get_total_num_devices()
+    cap = min(num_devices, args.num_layers)
+    if cap < 1 or cap > native.METIS_MAX_STAGES:
+        return None
+    variance, mpl = args.min_group_scale_variance, args.max_permute_len
+    try:
+        comps = flatten.count_compositions(num_devices, cap, variance, mpl)
+    except native.MetisNativeError:                           # beyond the counting table (more than 8192 GPUs)
+        return None
+    if comps <= _DEVICE_LISTING_COMPS:
+        return None
+    listing = listing_mod.DeviceListing(num_devices, cap, variance, mpl, dev, max_ranges=num_node_sequences * cap + 1)
+    return listing if listing.max_groups <= native.METIS_MAX_PERMUTE_GROUPS else None
+
+
+def _listed_windows(problem, space, listing, dev, rank: int, world: int):
+    """_het_windows for a space listed on the device: its windows (flatten.plan_listed_windows), a single one when the
+    whole space is searched at once."""
+    num_recs, _ = listing.size(flatten.whole_space_ranges(space))
+    windows = _het_windows(problem, space, dev, rank, world, num_recs=num_recs,
+                           plan=lambda budget, *model: flatten.plan_listed_windows(space, budget, *model, listing=listing))
+    if windows is None:
+        windows = flatten.plan_listed_windows(space, float('inf'), listing=listing)
+    return windows
 
 
 def _engine_bytes(key) -> int:
@@ -383,16 +437,19 @@ def _engine_bytes(key) -> int:
     return held
 
 
-def _het_windows(problem, space, dev, rank: int, world: int):
+def _het_windows(problem, space, dev, rank: int, world: int, num_recs: Optional[int] = None, plan=None):
     """None when ``space`` is searched by one metis_het_search call (today's path, the cached engine untouched), else
-    its windows (flatten.plan_windows), sized from the device memory free for them.  Every rank takes the smallest
-    budget of all ranks, so that all ranks make the same choice and cut the same windows."""
+    its windows (flatten.plan_windows, or ``plan(budget, per plan, per row byte, per record)``), sized from the device
+    memory free for them.  Every rank takes the smallest budget of all ranks, so that all ranks make the same choice
+    and cut the same windows.  ``num_recs``: the space's composition records when it does not hold them itself."""
     from . import search
-    if space.comp_recs is None:                               # host rows: build_plan_space kept its limits
+    if space.comp_recs is None and num_recs is None:          # host rows: build_plan_space kept its limits
         return None
+    if num_recs is None:
+        num_recs = len(space.comp_recs)
     per_plan, per_row, per_rec, fixed = search.window_cost_model(problem)
     shard = -(-space.num_plans // world) + 128                # plans of one rank's shard, with a tile of slack
-    need = shard * per_plan + int(space.rows_total_bytes) * per_row + len(space.comp_recs) * per_rec
+    need = shard * per_plan + int(space.rows_total_bytes) * per_row + num_recs * per_rec
     if flatten.fits_one_search(space) and need + fixed < _ONE_SEARCH_BYTES:
         return None
     key = (dev.index if dev.index is not None else -1, rank, world)
@@ -411,6 +468,8 @@ def _het_windows(problem, space, dev, rank: int, world: int):
     import torch
     torch.cuda.empty_cache()
     # a rank searches 1/world of each window's plans; the rows and composition records are whole on every rank
+    if plan is not None:
+        return plan(budget, per_plan / world, per_row, per_rec)
     return flatten.plan_windows(space, budget, per_plan / world, per_row, per_rec)
 
 

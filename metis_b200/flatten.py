@@ -464,22 +464,34 @@ class PlanWindow:
     def plan_at(self, ordinal: int) -> Tuple[int, int, int, int, int, int]:
         """Global ``ordinal`` -> (ns_idx, label_stage, dg_idx, batches, num_stage, byte offset of its row in the
         window's rows); dg_idx is the row in the whole space's table of that stage count, as in InterStagePlan."""
-        sp = self.space
-        rel = ordinal - self.base
-        if not 0 <= rel < sp.num_plans:
-            raise IndexError(f'ordinal {ordinal} is not in this window')
-        b = int(np.searchsorted(sp.blocks['first_ordinal'], rel, side='right')) - 1
-        blk = sp.blocks[b]
-        row, div = divmod(rel - int(blk['first_ordinal']), len(sp.batches))
-        S = int(blk['num_stage'])
-        return (int(blk['ns_idx']), int(blk['label_stage']), int(self.row_base[b]) + row, int(sp.batches[div]), S,
-                int(blk['rows_offset']) + row * S)
+        return _plan_at(self.base, self.space, self.row_base, ordinal)
 
     def locate(self, ordinal: int, rows: np.ndarray) -> Tuple[int, int, int, int, np.ndarray]:
         """Global ``ordinal`` -> (ns_idx, label_stage, dg_idx, batches, device_groups) like FlatPlanSpace.locate, with
         the codes read from ``rows`` (the window's row blob, e.g. generated on the host)."""
         ns, label, dg, batches, S, at = self.plan_at(ordinal)
         return ns, label, dg, batches, rows[at:at + S]
+
+    def arena_sizes(self) -> Dict[str, int]:
+        """Bytes of the space's tables in a DeviceProblem arena (search.search_windows sizes one arena for all)."""
+        return _arena_sizes(self.space, self.space.comp_recs.nbytes, self.space.comp_pool.nbytes)
+
+
+def _plan_at(base: int, sp: FlatPlanSpace, row_base: np.ndarray, ordinal: int) -> Tuple[int, int, int, int, int, int]:
+    rel = ordinal - base
+    if not 0 <= rel < sp.num_plans:
+        raise IndexError(f'ordinal {ordinal} is not in this window')
+    b = int(np.searchsorted(sp.blocks['first_ordinal'], rel, side='right')) - 1
+    blk = sp.blocks[b]
+    row, div = divmod(rel - int(blk['first_ordinal']), len(sp.batches))
+    S = int(blk['num_stage'])
+    return (int(blk['ns_idx']), int(blk['label_stage']), int(row_base[b]) + row, int(sp.batches[div]), S,
+            int(blk['rows_offset']) + row * S)
+
+
+def _arena_sizes(space: FlatPlanSpace, rec_bytes: int, pool_bytes: int) -> Dict[str, int]:
+    return dict(blocks=space.blocks.nbytes, batches=space.batches.nbytes, comp_recs=int(rec_bytes),
+                comp_pool=int(pool_bytes), rows=int(space.rows_total_bytes))
 
 
 def window_bytes(space: FlatPlanSpace, plan_bytes: float, row_bytes: float, rec_bytes: float) -> float:
@@ -660,3 +672,207 @@ def enumerate_compositions(first_stage: int, last_stage: int, num_gpus: int, var
     if got != ncomp:
         raise native.MetisNativeError('metis_enum_compositions: inconsistent count')
     return counts, recs[:int(ncomp)], pool, int(most.value)
+
+
+# ---------------------------------------------------------------------------------------------
+# device listing (SURVEY.md 8(f)-1): the GPU lists the compositions (metis_list_*, metis_b200.listing), the host plans
+# the windows from the rows of each stage count and holds one window's records at a time
+# ---------------------------------------------------------------------------------------------
+def count_compositions(num_devices: int, cap: int, variance, max_permute_len: int, lib=None) -> int:
+    """Compositions of stage counts 1..cap (what metis_enum_compositions would list), from the counting table of the
+    device listing; host only, no listing."""
+    lib = lib or native.load_library()
+    listing = native.MetisListing(1, cap, num_devices, max_permute_len, float(variance), 1, 0)
+    comps = np.zeros(cap, dtype=np.int64)
+    n = lib.metis_list_workspace_bytes(C.byref(listing), comps.ctypes.data)
+    if n < 0:
+        native.check(int(n), 'metis_list_workspace_bytes')
+    return int(comps.sum())
+
+
+def listed_plan_space(num_node_sequences: int, num_devices: int, gbs: int, num_layers: int, rows_per_stage,
+                      corrected: Sequence[str] = ()) -> FlatPlanSpace:
+    """The block list of a space whose compositions the GPU lists: ``rows_per_stage[S - 1]`` = rows of stage count S.
+    The space has no records (``comp_recs`` is None); plan_listed_windows cuts it into windows that get theirs."""
+    cap = min(num_devices, num_layers)
+    batches = [b for b in range(gbs, 0, -1) if gbs % b == 0]   # plan.py:120-124
+    nrows_of = lambda st: int(rows_per_stage[st - 1]) if 1 <= st <= min(cap, len(rows_per_stage)) else 0  # noqa: E731
+    offsets, off = {}, 0
+    for stages in range(1, cap + 1):
+        offsets[stages] = off
+        off += nrows_of(stages) * stages
+    plan_blocks = _walk_blocks(num_node_sequences, cap, nrows_of, corrected)
+    _check_stage_limit(plan_blocks)
+    blocks, total = _blocks_array(plan_blocks, nrows_of, lambda st: offsets[st], len(batches))
+    space = FlatPlanSpace(total, blocks, np.asarray(batches, dtype=np.int32), np.zeros(0, dtype=np.uint8))
+    space.rows_total_bytes = off
+    return space
+
+
+class ListedWindow:
+    """A window of a listed space (plan_listed_windows), with PlanWindow's interface: ``base``, ``row_base``,
+    ``plan_at`` / ``locate`` and ``space``, a FlatPlanSpace whose ``comp_recs`` / ``comp_pool`` are the window's own.
+    The records are written by the device listing when ``space`` is asked for (``emit(ranges)`` -> (recs, pool)); the
+    listing keeps the last window's only, so the host never holds more than one window's records."""
+
+    def __init__(self, base: int, layout: FlatPlanSpace, row_base: np.ndarray, ranges: np.ndarray, rec_bound: int,
+                 listing):
+        self.base = base
+        self.layout = layout          # blocks, batches, plans, rows; no records
+        self.row_base = row_base
+        self.ranges = ranges          # native.RANGE_DTYPE: the window's rows, range after range
+        self.rec_bound = rec_bound    # at most one record per row
+        self.listing = listing        # .window_space(window) -> FlatPlanSpace, .size(ranges) -> (records, pool bytes)
+        self.num_recs = self.pool_bytes = None
+
+    @property
+    def space(self) -> FlatPlanSpace:
+        return self.listing.window_space(self)
+
+    def plan_at(self, ordinal: int) -> Tuple[int, int, int, int, int, int]:
+        return _plan_at(self.base, self.layout, self.row_base, ordinal)
+
+    def locate(self, ordinal: int, rows: np.ndarray) -> Tuple[int, int, int, int, np.ndarray]:
+        ns, label, dg, batches, S, at = self.plan_at(ordinal)
+        return ns, label, dg, batches, rows[at:at + S]
+
+    def sized(self) -> 'ListedWindow':
+        """Ask the listing for the window's exact record count and pool size (no records written)."""
+        if self.num_recs is None:
+            self.num_recs, self.pool_bytes = self.listing.size(self.ranges)
+        return self
+
+    def arena_sizes(self) -> Dict[str, int]:
+        self.sized()
+        return _arena_sizes(self.layout, self.num_recs * np.dtype(native.COMP_DTYPE).itemsize, self.pool_bytes)
+
+
+def _row_union(ivs: List[Tuple[int, int]], a: int, e: int) -> List[Tuple[int, int]]:
+    out: List[Tuple[int, int]] = []
+    for x, y in sorted(ivs + [(a, e)]):
+        if out and x <= out[-1][1]:
+            out[-1] = (out[-1][0], max(out[-1][1], y))
+        else:
+            out.append((x, y))
+    return out
+
+
+def _new_rows(ivs: List[Tuple[int, int]], a: int, e: int) -> int:
+    """Rows of [a, e) outside the disjoint intervals ``ivs``."""
+    return (e - a) - sum(max(0, min(e, y) - max(a, x)) for x, y in ivs)
+
+
+def plan_listed_windows(space: FlatPlanSpace, budget: float, plan_bytes: float = 1.0, row_bytes: float = 0.0,
+                        rec_bytes: float = 0.0, listing=None) -> List[ListedWindow]:
+    """plan_windows for a listed space (listed_plan_space): windows in ordinal order, each within the limits of one
+    search, such that one arena sized for all of them fits ``budget`` under the same cost model, counting one
+    composition record per row (a record holds at least one row; the exact count is not known before the window is
+    listed).  Cuts fall on any row; a window holds at least one slice's rows (METIS_COMP_SLICE_ROWS), whatever the
+    budget.  Deterministic: every rank cuts the same windows from the same budget."""
+    target = budget
+    for _ in range(8):
+        windows = _cut_listed(space, target, plan_bytes, row_bytes, rec_bytes, listing)
+        peak = (max(w.layout.num_plans for w in windows) * plan_bytes
+                + max(int(w.layout.rows_total_bytes) for w in windows) * row_bytes
+                + max(w.rec_bound for w in windows) * rec_bytes)
+        if peak <= budget or target <= 0:
+            break
+        target = min(target * budget / peak, target - 1)
+    return windows
+
+
+METIS_COMP_SLICE_ROWS = 64
+
+
+def _cut_listed(space: FlatPlanSpace, budget: float, plan_bytes: float, row_bytes: float, rec_bytes: float,
+                listing) -> List[ListedWindow]:
+    ndiv = len(space.batches)
+    windows: List[ListedWindow] = []
+    seg: List[Tuple[int, int, int]] = []                  # (parent block, first row, end row)
+    covered: Dict[int, List[Tuple[int, int]]] = {}        # S -> disjoint row intervals of the window's rows
+    state = [0, 0, 0, 0]                                  # plans, row bytes, rows (record bound), base ordinal
+
+    def close():
+        windows.append(_listed_window(space, seg, covered, state[3], state[2], listing))
+        state[3] += state[0]
+        state[:3] = [0, 0, 0]
+        seg.clear()
+        covered.clear()
+
+    for b in range(len(space.blocks)):
+        S, n = int(space.blocks['num_stage'][b]), int(space.blocks['num_rows'][b])
+        r = 0
+        while r < n:
+            ivs = covered.get(S, [])
+
+            def fits(e: int) -> bool:
+                new = _new_rows(ivs, r, e)
+                plans, rows = state[0] + (e - r) * ndiv, state[1] + new * S
+                cost = plans * plan_bytes + rows * row_bytes + (state[2] + new) * rec_bytes
+                return plans <= MAX_SEARCH_PLANS and rows <= MAX_SEARCH_ROW_BYTES and cost <= budget
+
+            if fits(n):
+                fit = n
+            else:                                         # largest end row that fits (the cost grows with it)
+                lo, hi = r, n
+                while hi - lo > 1:
+                    mid = (lo + hi) // 2
+                    if fits(mid):
+                        lo = mid
+                    else:
+                        hi = mid
+                fit = lo
+            if fit == r:
+                if seg:                                   # nothing more fits: the next window starts here
+                    close()
+                    continue
+                fit = min(n, r + METIS_COMP_SLICE_ROWS)   # an empty window takes one slice
+            new = _new_rows(ivs, r, fit)
+            state[0] += (fit - r) * ndiv
+            state[1] += new * S
+            state[2] += new
+            seg.append((b, r, fit))
+            covered[S] = _row_union(ivs, r, fit)
+            r = fit
+            if r < n:
+                close()
+    if seg:
+        close()
+    return windows
+
+
+def _listed_window(space: FlatPlanSpace, seg, covered, base: int, rec_bound: int, listing) -> ListedWindow:
+    ndiv = len(space.batches)
+    ranges = np.zeros(sum(len(v) for v in covered.values()), dtype=native.RANGE_DTYPE)
+    at: Dict[Tuple[int, int], int] = {}                   # (S, interval start) -> byte offset in the window's rows
+    k = off = 0
+    for S in sorted(covered):
+        for a, e in covered[S]:
+            ranges[k] = (S, 0, a, e)
+            at[(S, a)] = off
+            off += (e - a) * S
+            k += 1
+    blocks = np.zeros(len(seg), dtype=native.BLOCK_DTYPE)
+    row_base = np.zeros(len(seg), dtype=np.int64)
+    ordinal = 0
+    for i, (b, r0, r1) in enumerate(seg):
+        src = space.blocks[b]
+        S = int(src['num_stage'])
+        a = next(a for a, e in covered[S] if a <= r0 and r1 <= e)
+        blocks[i] = src
+        blocks[i]['first_ordinal'] = ordinal
+        blocks[i]['rows_offset'] = at[(S, a)] + (r0 - a) * S
+        blocks[i]['num_rows'] = r1 - r0
+        row_base[i] = r0
+        ordinal += (r1 - r0) * ndiv
+    layout = FlatPlanSpace(ordinal, blocks, space.batches, np.zeros(0, dtype=np.uint8))
+    layout.rows_total_bytes = off
+    return ListedWindow(base, layout, row_base, ranges, rec_bound, listing)
+
+
+def whole_space_ranges(space: FlatPlanSpace) -> np.ndarray:
+    """native.RANGE_DTYPE: every row of every stage count the blocks of ``space`` use, in stage-count order (the layout
+    of a one-window listed space)."""
+    stages = sorted({int(S) for S in space.blocks['num_stage']})
+    rows = {int(b['num_stage']): int(b['num_rows']) for b in space.blocks}
+    return np.array([(S, 0, 0, rows[S]) for S in stages], dtype=native.RANGE_DTYPE)

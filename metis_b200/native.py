@@ -67,6 +67,12 @@ class MetisShard(C.Structure):
     _fields_ = [('rank', C.c_int32), ('world', C.c_int32), ('tile', C.c_int32), ('reserved', C.c_int32)]
 
 
+class MetisListing(C.Structure):
+    _fields_ = [('first_stage', C.c_int32), ('last_stage', C.c_int32), ('num_gpus', C.c_int32),
+                ('max_permute_len', C.c_int32), ('variance', C.c_double), ('max_ranges', C.c_int32),
+                ('reserved', C.c_int32)]
+
+
 assert C.sizeof(MetisRecord) == 16 and C.sizeof(MetisPlanBlock) == 32
 
 # numpy dtype twins of the C structs
@@ -76,11 +82,13 @@ BLOCK_DTYPE = [('first_ordinal', '<i8'), ('rows_offset', '<i8'), ('num_rows', '<
 
 COMP_DTYPE = [('row_offset', '<i8'), ('pool_offset', '<u4'), ('stages', '<u2'), ('num_groups', '<u2'),
               ('first_row', '<u4'), ('num_rows', '<u4')]
+RANGE_DTYPE = [('stages', '<i4'), ('reserved', '<i4'), ('first_row', '<i8'), ('end_row', '<i8')]   # MetisRowRange
 
 SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 'metis_het_workspace_bytes', 'metis_het_search',
            'metis_het_detail', 'metis_het_trace', 'metis_homo_cost', 'metis_layer_balance', 'metis_enum_device_groups',
            'metis_enum_device_group_tables', 'metis_sort_workspace_bytes', 'metis_sort_records',
-           'metis_enum_compositions', 'metis_generate_rows']
+           'metis_enum_compositions', 'metis_generate_rows', 'metis_list_workspace_bytes', 'metis_list_stages',
+           'metis_list_window']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -132,6 +140,13 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
                                             C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.metis_generate_rows.restype = C.c_int
     lib.metis_generate_rows.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.metis_list_workspace_bytes.restype = C.c_int64
+    lib.metis_list_workspace_bytes.argtypes = [C.POINTER(MetisListing), C.c_void_p]
+    lib.metis_list_stages.restype = C.c_int
+    lib.metis_list_stages.argtypes = [C.POINTER(MetisListing), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.metis_list_window.restype = C.c_int
+    lib.metis_list_window.argtypes = [C.POINTER(MetisListing), C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p,
+                                      C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.metis_sort_workspace_bytes.restype = C.c_int64
     lib.metis_sort_workspace_bytes.argtypes = [C.c_int64]
     lib.metis_sort_records.restype = C.c_int

@@ -43,9 +43,9 @@ class DeviceProblem:
     host -> device copy; ``reload`` puts another problem / space of compatible size into the same buffers."""
 
     def __init__(self, problem: flatten.FlatProblem, space: flatten.FlatPlanSpace, device=None,
-                 pinned: bool = True, rows_capacity: int = 0, reserve: Sequence[flatten.FlatPlanSpace] = ()):
-        """``reserve``: further spaces (the windows of a windowed search) the arena is sized for up front, so that
-        reloading any of them reuses the buffers."""
+                 pinned: bool = True, rows_capacity: int = 0, reserve: Sequence = ()):
+        """``reserve``: the windows of a windowed search (flatten.PlanWindow / ListedWindow, ``arena_sizes()``) the
+        arena is sized for up front, so that reloading any of them reuses the buffers."""
         self.device = _require_cuda(device)
         self.lib = native.load_library()
         self.pinned = pinned
@@ -53,10 +53,9 @@ class DeviceProblem:
         self._off: Dict[str, Tuple[int, int]] = {}           # name -> (offset, capacity)
         self._used: Dict[str, int] = {}
         self._reserve: Dict[str, int] = {}
-        for s in reserve:
-            flat = self._arrays(problem, s)
-            for name in _ARENA_ORDER:
-                self._reserve[name] = max(self._reserve.get(name, 0), self._need(flat, s, name))
+        for w in reserve:
+            for name, n in w.arena_sizes().items():
+                self._reserve[name] = max(self._reserve.get(name, 0), n)
         self._allocate(self._arrays(problem, space), space, rows_capacity)
         self.reload(problem, space)
         self.upload()
@@ -576,7 +575,7 @@ def search_windows(problem: flatten.FlatProblem, windows: Sequence[flatten.PlanW
     HetSearcher (the shard's tiles of every window, workspace sized for the window with the most plans), records only,
     and merge on the host (WindowMerge).  Afterwards the searcher keeps only what rebuilding candidates needs
     (metis_het_detail's workspace): the work lists and the record buffer are released."""
-    dp = DeviceProblem(problem, windows[0].space, device, reserve=[w.space for w in windows])
+    dp = DeviceProblem(problem, windows[0].space, device, reserve=windows)
     searcher = HetSearcher(dp, rank, world, tile, want_records=True, want_detail=False)
     searcher.reserve_workspace(max(w.space.num_plans for w in windows))
     merge = WindowMerge(len(windows))
