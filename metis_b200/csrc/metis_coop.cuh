@@ -99,7 +99,7 @@ MB_HD int par_index(const OneLane &x, int i, int n) { return x.reverse ? n - 1 -
 // ---------------------------------------------------------------------------------------------------------
 // Sequential pieces of LayerComputeBalancer.run (model/load_balancer.py:216-287) for the leader lane: the
 // compare-and-subtract chains in fp64.  Same state encoding as balance_run in metis_eval.cuh (fe[] interval ends
-// with kBroke / kTaken, lstk[], the per-layer packed stage map subw[]).
+// with kBroke / kTaken, lstk[], the middle block's stages in subw[]).
 // ---------------------------------------------------------------------------------------------------------
 struct FillState {
     int k;          // first sub-layer not offered to a forward stage

@@ -152,6 +152,7 @@ enum BalancerPath {
     kPathMiddle = 3,         // sub-layers are left between the forward and backward passes (the middle block)
     kPathFirstGe = 4,        // coop: a prediction missed its 32-entry window and searched the whole table
     kPathTail = 5,           // the forward pass ran into the reserved last 8 sub-layers with stages to spare
+    kPathVoteEnds = 6,       // balance_run: the vote took a forward sub-layer's stage from the interval ends fe[]
 };
 
 // Policies of PlanEvaluator and balance_run, which always evaluate one plan in one thread.  `Serial`: the thread
@@ -165,6 +166,28 @@ struct Serial {
     MB_HD void converge() const {}
     MB_HD void rejoin(bool) {}
 };
+#if defined(__CUDACC__) && defined(METIS_PROFILE_PHASES)
+// Phase clock of the bulk round (tools/phase_profile.py --bulk), read with metis_debug_bulk_marks.  Per warp, the
+// cycles from one hook (DeviceSink::phase, Lockstep::mark) to the next are added to the slot of the earlier hook's id
+// by the lowest lane of the warp's current group; phase(1) starts a batch of 32 plans (the fetch before it is not
+// counted) and slot kBulkBatches counts the batches.
+constexpr int kBulkBatches = 31;
+__device__ long long g_bulk_acc[32];
+__shared__ long long s_bulk_t[32];
+__shared__ int s_bulk_cur[32];
+__device__ __forceinline__ void bulk_mark(unsigned group, int id) {   // called by every lane of `group`
+    __syncwarp(group);
+    if ((int)(threadIdx.x & 31) == __ffs((int)group) - 1) {
+        const int wi = threadIdx.x >> 5;
+        const long long now = clock64();
+        if (id == 1) atomicAdd((unsigned long long *)&g_bulk_acc[kBulkBatches], 1ULL);
+        else atomicAdd((unsigned long long *)&g_bulk_acc[s_bulk_cur[wi] & 31], (unsigned long long)(now - s_bulk_t[wi]));
+        s_bulk_cur[wi] = id;
+        s_bulk_t[wi] = now;
+    }
+    __syncwarp(group);
+}
+#endif
 #if defined(__CUDACC__)
 // `Lockstep`: the bulk round of the search (metis_search.cu, het_first_kernel) - the 32 lanes of a warp hold 32
 // different plans of equal stage count and should execute the same instruction stream.  Data-dependent branches
@@ -177,6 +200,9 @@ struct Lockstep : Serial {
     __device__ Lockstep() : mask(0xFFFFFFFFu) {}
     __device__ void converge() const { __syncwarp(mask); }
     __device__ void rejoin(bool p) { mask = __ballot_sync(0xFFFFFFFFu, p); }
+#if defined(METIS_PROFILE_PHASES)
+    __device__ void mark(int id) const { bulk_mark(__activemask(), id); }   // mark(21): only the lanes out of memory
+#endif
 };
 #endif
 // `SerialUniform`: the base PlanEvaluator of the chain evaluator (metis_coop.cuh), whose per-stage members run in the
@@ -208,9 +234,9 @@ struct Scratch {
     uint8_t lstk[MAXS];    // stage on which the skipped sub-layer of stage s was placed
     uint8_t got[MAXS];     // stage received a leftover sub-layer
     uint64_t ownerw[MAXL / 8 + 1];   // byte r = stage owning real layer r after the vote (kDropped = none)
-    uint64_t subw[MAXL];   // per real layer: byte q = stage of sub-layer 7r+q (below the backward tail); the chain
-                           // evaluator keeps the stages of the middle block here instead (byte j - k, up to 7 * MAXL)
-    static_assert(MAXL >= MAXS, "after the vote, subw holds one double per stage (adjust_performance, get_cost)");
+    uint64_t subw[MAXL];   // byte j - k = stage of sub-layer j of the middle block (up to 7 * MAXL); the other
+                           // sub-layers' stages follow from fe[] and lstk[]
+    static_assert(MAXL >= MAXS, "after the vote, subw holds one double per stage (CoopEvaluator's adjust and cost)");
 };
 
 // ---------------------------------------------------------------------------
@@ -376,10 +402,6 @@ MB_HD bool fwd_nonempty(const Scratch<MAXS, MAXL> &w, int s) {
     return (int)(w.fe[s] & kPos) > fwd_start(w, s);
 }
 
-MB_HD void sub_store(uint64_t *subw, int j, int stage) {
-    reinterpret_cast<uint8_t *>(subw)[(j / kH) * 8 + (j % kH)] = (uint8_t)stage;
-}
-
 MB_HD int popc64(uint64_t v) {
 #if defined(__CUDA_ARCH__)
     return __popcll(v);
@@ -471,48 +493,44 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
                                                              // the lanes of the bulk round from re-joining (Lockstep)
 
 #pragma unroll (X::kUniform ? 1 : 0)
-    for (int s = 0; s < S; ++s) { w.capa[s] = w.perf[s]; w.got[s] = 0; w.cnt[s] = 0; }
+    for (int s = 0; s < S; ++s) { w.got[s] = 0; w.cnt[s] = 0; }
 
     x.mark(10);
     // ---- forward pass (:216-231): flat scan, layer by layer, 7 sub-layers each -----------------
+    // Each stage starts from its performance w.perf[s]; only the interval ends fe[] and the residual capacities of the
+    // stages it closes are written.  Which stage owns a sub-layer follows from fe[] (the vote below).
     int k = 0, sTop = -1;
     bool topSkip = false;
     if (S > 1) {
         int s = 0, j = 0;
-        double c = w.capa[0];
+        double c = w.perf[0];
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int r = 0; r + 1 < L; ++r) {
             const double d = dlay[r];
             const int nsub = (r == L - 2) ? kH - 1 : kH;     // the last 8 sub-layers are reserved
-            // one plan per thread: the layer's packed stage word is built in registers and stored once (the skipped
-            // sub-layers' bytes are filled in by the leftover pass below)
-            const int s_in = s;
-            uint64_t v = 0;
 #pragma unroll
             for (int q = 0; q < kH; ++q) {
                 if (q < nsub) {
                     if (s < last) {
                         if (c > d) {
                             c -= d;
-                            v |= (uint64_t)(uint32_t)s << (8 * q);
                         } else {                                 // sub-layer j does not fit: skipped, stage closes
                             w.capa[s] = c;
                             w.fe[s] = (uint16_t)(j | kBroke);
                             ++s;
-                            c = w.capa[s];
+                            c = w.perf[s];
                         }
                     }
                     ++j;
                 }
             }
-            if (s_in < last) w.subw[r] = v;
         }
         if (s < last) {                                          // ran into the reserved tail
             x.note(kPathTail);
             w.capa[s] = c;
             w.fe[s] = (uint16_t)lim;
 #pragma unroll (X::kUniform ? 1 : 0)
-            for (int t = s + 1; t < last; ++t) w.fe[t] = (uint16_t)lim;
+            for (int t = s + 1; t < last; ++t) { w.capa[t] = w.perf[t]; w.fe[t] = (uint16_t)lim; }
             k = lim;
             sTop = s;
         } else {
@@ -527,7 +545,7 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
     // ---- backward pass (:233-249): last stage takes a contiguous tail [m, N) -----------------
     int m;
     {
-        double c = w.capa[last];
+        double c = w.perf[last];
         const double dl = dlay[L - 1];
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int i = 0; i < kH; ++i) c -= dl;               // unconditional while len < hallucination (:237-241)
@@ -597,13 +615,13 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
             w.capa[pick] -= dlay[j / kH];
             w.lstk[s] = (uint8_t)pick;
             w.got[pick] = 1;
-            sub_store(w.subw, j, pick);
             start = next_start;
         }
     }
     x.converge();
-    const int nblk = m - k;                                   // any length up to 7 * L: the picks go to subw
+    const int nblk = m - k;                                   // any length up to 7 * L: pick t goes to byte t of subw
     if (nblk > 0) x.note(kPathMiddle);
+    uint8_t *mid = reinterpret_cast<uint8_t *>(w.subw);
     {
         int below = -1;                                       // stage of the nearest block item not on `last`
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -632,30 +650,45 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
                 if (w.capa[t2] > best) { best = w.capa[t2]; pick = t2; }
             w.capa[pick] -= dlay[j / kH];
             if (pick != last) below = pick;
-            sub_store(w.subw, j, pick);
+            mid[t] = (uint8_t)pick;
         }
     }
 
     x.mark(13);
     x.converge();
     // ---- majority vote back to real layers (:290-308) ------------------------------------------
+    // Stage of sub-layer j, from the interval ends: j >= m -> last stage (backward tail); k <= j < m -> where the
+    // middle block put it (byte j - k of subw); below k the forward slot t whose interval [start_t, nxt) holds j, and
+    // if j is that slot's skipped sub-layer (nxt - 1 with kBroke): the last stage when the backward pass took it, else
+    // where the leftover pass placed it (lstk).  The slot only moves up, one interval end at a time.
     // A stage holding >= 4 of a layer's 7 sub-layers holds the middle one or one of the first
     // three, so at most four candidates are counted (SWAR byte compare on the packed layer word).
+    if (k > 0) x.note(kPathVoteEnds);
+    int t = 0, nxt = 0;
+    uint16_t e = 0;
+    if (k > 0) { e = w.fe[0]; nxt = (int)(e & kPos) + ((e & kBroke) ? 1 : 0); }
+    const bool plurality = (T.p.corrected & METIS_FIX_Q5) != 0;
     int run_own = (int)kDropped, run_first = 0, run_len = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
     for (int r = 0; r < L; ++r) {
-        const int nlow = m - kH * r;                         // sub-layers of r below the backward tail
-        int own;
-        if (nlow <= 0) {
-            own = last;
-        } else {
-            uint64_t v = w.subw[r];
-            if (nlow < kH) {
-                const uint64_t mask = (1ULL << (8 * nlow)) - 1ULL;
-                v = (v & mask) | (((uint64_t)last * kOnes) & ~mask);
+        int own = last;
+        if (kH * r < m) {
+            uint64_t v = 0xFF00000000000000ULL;
+#pragma unroll
+            for (int q = 0; q < kH; ++q) {
+                const int j = kH * r + q;
+                int st = last;
+                if (j < k) {
+#pragma unroll 1
+                    while (nxt <= j) { ++t; e = w.fe[t]; nxt = (int)(e & kPos) + ((e & kBroke) ? 1 : 0); }
+                    st = t;
+                    if (nxt - 1 == j && (e & kBroke)) st = (e & kTaken) ? last : (int)w.lstk[t];
+                } else if (j < m) {
+                    st = mid[j - k];
+                }
+                v |= (uint64_t)(uint32_t)st << (8 * q);
             }
-            v |= 0xFF00000000000000ULL;
-            own = layer_owner(v, (T.p.corrected & METIS_FIX_Q5) != 0);
+            own = layer_owner(v, plurality);
         }
         reinterpret_cast<uint8_t *>(w.ownerw)[r] = (uint8_t)own;
         {
@@ -679,20 +712,22 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
     x.mark(14);
     x.converge();
     uint8_t *owner = reinterpret_cast<uint8_t *>(w.ownerw);
+    // spare capacity (:300-306), with the arg-max of the first adjustment round (stable: lowest index among equal
+    // maxima, :329-331); a committed round finds the next round's arg-max while it checks its new maximum
+    int top = 0x7FFFFFFF;
+    double maxc = -INFINITY;
 #pragma unroll (X::kUniform ? 1 : 0)
-    for (int s = 0; s < S; ++s)                              // :300-306
-        w.capa[s] = w.cnt[s] ? w.perf[s] - range_sum<X>(T, kRangeNorm, 0, lc, w.first[s], (int)w.lastl[s] + 1) : w.perf[s];
+    for (int s = 0; s < S; ++s) {
+        const double c = w.cnt[s] ? w.perf[s] - range_sum<X>(T, kRangeNorm, 0, lc, w.first[s], (int)w.lastl[s] + 1) : w.perf[s];
+        w.capa[s] = c;
+        if (c > maxc) { maxc = c; top = s; }
+    }
 
     x.mark(15);
     x.converge();
     // ---- boundary adjustment (:310-356): at most three committed single-layer moves ---------
 #pragma unroll (X::kUniform ? 1 : 0)
     for (int n = 1; n <= 3; ++n) {
-        int top = 0x7FFFFFFF;
-        double maxc = -INFINITY;
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int t = 0; t < S; ++t)                          // stable: lowest index among equal maxima (:329-331)
-            if (w.capa[t] > maxc) { maxc = w.capa[t]; top = t; }
         if (top == 0x7FFFFFFF) top = 0;
         int nb = -1;
         double val = INFINITY;
@@ -704,10 +739,11 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
         const double ntop = w.capa[top] - dl;
         const double nnb = w.capa[nb] + dl;
         double newmax = -INFINITY;
+        int newtop = 0x7FFFFFFF;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int t = 0; t < S; ++t) {
             const double v = (t == top) ? ntop : (t == nb) ? nnb : w.capa[t];
-            if (v > newmax) newmax = v;
+            if (v > newmax) { newmax = v; newtop = t; }
         }
         if (newmax > maxc) break;                            // :352 (not committed)
         owner[layer] = (uint8_t)top;
@@ -722,6 +758,8 @@ MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x
         }
         ++w.cnt[top];
         --w.cnt[nb];
+        maxc = newmax;                                       // the next round's arg-max: the committed capacities
+        top = newtop;
     }
 
     x.mark(16);
@@ -1108,24 +1146,24 @@ struct PlanEvaluator {
         upd = T.p.optimizer_time * inv_tp * T.ratio[lb - la];   // :145-147
     }
 
-    // ---- Sequential drivers of the cost model (one plan per thread).
+    // ---- Sequential drivers of the cost model (one plan per thread).  One thread walks the stages in order, so the
+    // first failing stage ends a loop with its code and `aux` in registers, and the order-dependent sums are taken
+    // in the same pass as the values they add up.
 
     // StagePerformance.get_intra_stage_compute_performance (model/device_group.py:54-85) -> w.perf
     MB_HD int compute_performance() {
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = 0; s < pd.S; ++s) {
-            double p;
-            const int rc = stage_performance(s, p);
-            w.perf[s] = p;
-            w.extra[s] = encode_error(rc, aux);
-        }
-        x.converge();
         PySum total;
+        int rc = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int s = 0; s < pd.S; ++s) {                     // first failing stage in stage order, like the reference
-            if (w.extra[s] != 0.0) return decode_error(w.extra[s], aux);
-            total.add(w.perf[s]);
+            double p;
+            rc = stage_performance(s, p);
+            if (rc) break;
+            w.perf[s] = p;
+            total.add(p);
         }
+        x.converge();
+        if (rc) return rc;
         const double tot = total.result();
         if (tot == 0.0) return METIS_FATAL_ZERODIV;
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -1197,9 +1235,9 @@ struct PlanEvaluator {
 
     // LayerLoadBalancer._adj_compute_performance (model/load_balancer.py:71-107)
     // in: w.perf (c_capa), w.extra (m_demand); out: w.perf; returns 1 = None, 0 ok, <0 fatal (negated code)
+    // w.extra is overwritten on both returns (additional_alloc_sc_capa; zero when the result is None)
     MB_HD_NOINLINE int adjust_performance() {
         const int S = pd.S;
-        double *ratio = reinterpret_cast<double *>(w.subw);      // free after the vote (MAXL >= MAXS)
         double need = 0.;
         PySum avail_sum;
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -1208,12 +1246,11 @@ struct PlanEvaluator {
             stage_adjust(s, av, adj, extra);
             w.capa[s] = av;           // available_compute_capacity
             w.mstate[s] = adj;        // adj_sc_capa
+            w.extra[s] = 0.;          // the demand is read: the additional allocation starts here
             need += extra;
             avail_sum.add(av);
         }
         if (avail_sum.result() < need) return 1;
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = 0; s < S; ++s) w.extra[s] = 0.;
         int guard = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
         while (need > 0.01) {
@@ -1222,12 +1259,12 @@ struct PlanEvaluator {
             for (int s = 0; s < S; ++s) tot.add(w.capa[s] > 0.001 ? w.perf[s] : 0.0);
             const double tmp_total = tot.result();
 #pragma unroll (X::kUniform ? 1 : 0)
-            for (int s = 0; s < S; ++s)                          // c_capa_ratio list (:98), before the updates
-                ratio[s] = w.capa[s] > 0.001 ? w.perf[s] / tmp_total : 0.0;
-#pragma unroll (X::kUniform ? 1 : 0)
             for (int s = 0; s < S; ++s) {                        // :100-104, sequential: `need` changes as it goes
                 const double av = w.capa[s];
-                const double want = need * ratio[s];
+                // c_capa_ratio (:98) is taken before the updates; stage s's entry depends on stage s alone, which
+                // no earlier update touches
+                const double ratio = av > 0.001 ? w.perf[s] / tmp_total : 0.0;
+                const double want = need * ratio;
                 const double give = want > av ? av : want;
                 w.extra[s] += give;
                 w.capa[s] -= give;
@@ -1248,32 +1285,26 @@ struct PlanEvaluator {
     // call is skipped here.
     MB_HD int memory_phase(int attempt) {
         const int S = pd.S;
+        bool oom = false;
+        int rc = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = 0; s < S; ++s) {
+        for (int s = 0; s < S; ++s) {                        // first failing stage in stage order, like the reference
             double md, state;
-            const int rc = stage_memory(s, md, state);
+            rc = stage_memory(s, md, state);
+            if (rc) break;
             w.extra[s] = md;
-            w.capa[s] = state;
-            w.mstate[s] = encode_error(rc, aux);
+            w.mstate[s] = state;
+            if (state < 0) oom = true;
             if (tap) { tap->demand[s] = md; tap->state[s] = state; }
         }
         x.converge();
-        bool oom = false;
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = 0; s < S; ++s) {
-            if (w.mstate[s] != 0.0) return -decode_error(w.mstate[s], aux);
-            if (w.capa[s] < 0) oom = true;
-        }
-        if (!oom) {
-#pragma unroll (X::kUniform ? 1 : 0)
-            for (int s = 0; s < S; ++s) w.mstate[s] = w.capa[s];
-            return 1;
-        }
+        if (rc) return -rc;
+        if (!oom) return 1;
         if (attempt >= 3) return 0;
         x.mark(21);
-        const int rc = adjust_performance();
-        if (rc < 0) return rc;
-        return rc == 1 ? 0 : 2;
+        const int adj = adjust_performance();
+        if (adj < 0) return adj;
+        return adj == 1 ? 0 : 2;
     }
 
     // LayerLoadBalancer.partition_layer (model/load_balancer.py:121-144)
@@ -1394,31 +1425,28 @@ struct PlanEvaluator {
         // rank_node_map holds num_nodes * devices(node 0) ranks (cluster_bandwidth.py:34-47, Q10): a costed stage
         // (or its pipeline successor) beyond that raises KeyError -> the candidate is skipped
         if (T.p.q10_devices < T.p.total_devices && rank_start(nstage) > T.p.q10_devices) return 1;
-        // execution time of every stage first (w.capa[s]); the terms only when no stage raised a KeyError
+        // execution time of every stage first; the terms only when no stage raised a KeyError.  The order-dependent
+        // sums run in stage order inside the two loops, so nothing is stored per stage.
         bool bad = false;
+        PySum lens_sum;
+        double max_len = -INFINITY;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int s = 0; s < nstage; ++s) {
             double len;
             if (stage_time(s, len)) bad = true;
-            w.capa[s] = len;
+            lens_sum.add(len);
+            if (len > max_len) max_len = len;
         }
         if (bad) return 1;                                    // KeyError raised while costing a stage
-        double *ppterm = reinterpret_cast<double *>(w.subw);  // free after the vote (MAXL >= MAXS)
-        double max_len = -INFINITY, max_upd = -INFINITY, max_dp = -INFINITY;
-#pragma unroll (X::kUniform ? 1 : 0)
-        for (int s = 0; s < nstage; ++s) {
-            double dpc, upd;
-            stage_terms(s, nstage, ppterm[s], dpc, upd);
-            if (w.capa[s] > max_len) max_len = w.capa[s];
-            if (dpc > max_dp) max_dp = dpc;
-            if (upd > max_upd) max_upd = upd;
-        }
-        PySum lens_sum;                                       // order-dependent sums, stage order
+        double max_upd = -INFINITY, max_dp = -INFINITY;
         double pp_cost = 0., fb_sync = 0.;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int s = 0; s < nstage; ++s) {
-            lens_sum.add(w.capa[s]);
-            if (s < nstage - 1) pp_cost += ppterm[s];
+            double pp, dpc, upd;
+            stage_terms(s, nstage, pp, dpc, upd);
+            if (s < nstage - 1) pp_cost += pp;
+            if (dpc > max_dp) max_dp = dpc;
+            if (upd > max_upd) max_upd = upd;
         }
         {
             const int s = nstage - 1;                         // _get_fb_sync_cost of the last costed stage

@@ -290,7 +290,11 @@ struct DeviceSink {
     __device__ DeviceSink(const DeviceOut &out)
         : o(out), n_part(0), n_run(0), n_key(0), best_cost(INFINITY), best_ord(0xFFFFFFFFu), best_step(0xFFFFu),
           best_meta(0), leader(true) {}
+#ifdef METIS_PROFILE_PHASES
+    __device__ void phase(int id) { bulk_mark(0xFFFFFFFFu, id); }   // bulk round: called by all 32 lanes
+#else
     __device__ void phase(int) {}
+#endif
     __device__ void partition_call() { n_part += leader ? 1u : 0u; }
     __device__ void balancer_run() { n_run += leader ? 1u : 0u; }
     __device__ void keyerror() { n_key += leader ? 1u : 0u; }
@@ -804,6 +808,12 @@ int metis_debug_marks(long long *out32, int reset) {
     long long zero[64] = {0};
     if (out32) cudaMemcpyFromSymbol(out32, g_mark_acc, sizeof(zero));      // caller provides 64 entries
     if (reset) cudaMemcpyToSymbol(g_mark_acc, zero, sizeof(zero));
+    return 0;
+}
+int metis_debug_bulk_marks(long long *out32, int reset) {
+    long long zero[32] = {0};
+    if (out32) cudaMemcpyFromSymbol(out32, g_bulk_acc, sizeof(zero));      // caller provides 32 entries
+    if (reset) cudaMemcpyToSymbol(g_bulk_acc, zero, sizeof(zero));
     return 0;
 }
 #endif

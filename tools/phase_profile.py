@@ -10,7 +10,11 @@ reads clock64() on the leader lane of every warp at each phase mark (metis_coop.
 block gate (ChainCoop::gate).  Printed per phase: share of the chain warps' cycles and cycles per balancer run of
 the chain kernel (total cycles of the phase over the runs; the time a warp spends waiting in a gate is the phase
 `gate wait`), and the histogram of the gate spread: per block and gate, the cycles from the first working warp's
-arrival to the last one's, i.e. how long the fastest warp waits for the slowest."""
+arrival to the last one's, i.e. how long the fastest warp waits for the slowest.
+
+--bulk prints the bulk round (het_first_kernel) instead: its phase clock runs on the lowest lane of each warp's
+current group from one hook (DeviceSink::phase, Lockstep::mark) to the next.  Printed per phase: share of the bulk
+round's warp-cycles, cycles per batch of 32 plans (one warp in lockstep) and per plan (a batch's cycles / 32)."""
 import argparse
 import ctypes
 import itertools
@@ -31,18 +35,34 @@ NAMES = {0: 'fetch+decode', 1: 'begin+strategy', 2: 'P perf', 9: 'R init', 10: '
          16: 'R part', 20: 'M demand', 21: 'M reweight', 22: 'C stage terms', 23: 'C sums+emit', 24: 'chain advance',
          25: 'drain', 30: 'gate wait'}
 RUNS, GATES, SPREAD, WARPS, HIST = 32, 33, 34, 35, 40     # WarpCoop's kMark* slots
+BULK_NAMES = {1: 'P performance', 2: 'R init', 10: 'R forward', 11: 'R backward', 12: 'R leftovers', 13: 'R vote',
+              14: 'R capacities', 15: 'R adjust', 16: 'R part', 3: 'M memory', 21: 'M reweight', 4: 'C cost'}
+BULK_BATCHES = 31                                         # kBulkBatches (metis_eval.cuh)
+
+
+def print_bulk(name, ms, marks):
+    batches = marks[BULK_BATCHES] or 1
+    tot = sum(marks[i] for i in BULK_NAMES) or 1
+    print(f'{name}: {ms:.2f} ms (phase-clock build), bulk round: {marks[BULK_BATCHES]} batches of 32 plans, '
+          f'{tot / 1e6:.1f} M warp-cycles, {tot / batches:.0f} per batch')
+    print(f'  {"phase":<16s} {"share":>7s} {"cycles/batch":>13s} {"cycles/plan":>12s}')
+    for i in BULK_NAMES:
+        print(f'  {BULK_NAMES[i]:<16s} {100.0 * marks[i] / tot:6.1f}% {marks[i] / batches:13.0f} '
+              f'{marks[i] / batches / 32:12.1f}')
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('workload', nargs='?', default='c3_homo64_mpl6')
     ap.add_argument('--build', action='store_true', help='build libmetis_b200_prof.so first')
+    ap.add_argument('--bulk', action='store_true', help='the bulk round (het_first_kernel) instead of the chain kernel')
     ns = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('phase_profile.py needs a CUDA device')
     prof = build.build_library(profile=True) if ns.build else build.PROF_LIB
     native._lib = native.load_library(prof)
     native._lib.metis_debug_marks.argtypes = [ctypes.c_void_p, ctypes.c_int]
+    native._lib.metis_debug_bulk_marks.argtypes = [ctypes.c_void_p, ctypes.c_int]
     w = WORKLOADS[ns.workload]
     tmp = tempfile.mkdtemp()
     materialize(w, tmp)
@@ -62,9 +82,15 @@ def main():
     torch.cuda.synchronize()
     marks = (ctypes.c_longlong * 64)()
     native._lib.metis_debug_marks(None, 1)
+    native._lib.metis_debug_bulk_marks(None, 1)
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record(); s.launch(); b.record(); torch.cuda.synchronize()
     sm = s.summary()
+    if ns.bulk:
+        bulk = (ctypes.c_longlong * 32)()
+        native._lib.metis_debug_bulk_marks(ctypes.addressof(bulk), 0)
+        print_bulk(ns.workload, a.elapsed_time(b), bulk)
+        return
     native._lib.metis_debug_marks(ctypes.addressof(marks), 0)
     mt = sum(marks[:32]) or 1
     runs = marks[RUNS] or 1
