@@ -466,20 +466,27 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
             a = closed ? b + 1 : lim;
         }
         x.sync();
+        x.mark(19);
         // ---- exact replay of every stage from its predicted start ----
+        // The trip count is the predicted interval, so the loop has no exit: a compare that fails only clears `fits`
+        // (the reference would have closed the stage there), and the subtractions go on; c is then wrong, but a
+        // failed stage sends the whole pass to the sequential fallback, which restores capa.  Without the exit a
+        // sub-layer costs a load, a compare folded into the predicate and a subtraction instead of two branches and
+        // a byte-sized flag (the chain kernel pays for instructions issued, §5 of DESIGN.md).
         bool bad = false;
         METIS_PAR(x, s, last) {
             const int st = w.first[s];
             const uint16_t e = w.fe[s];
             const int b = e & kPos;
             double c = w.perf[s];
+            bool fits = true;
 #pragma unroll 4
             for (int j = st; j < b; ++j) {
                 const double d = dsub[j];
-                if (!(c > d)) { bad = true; break; }          // the reference would have closed the stage here
+                fits &= c > d;
                 c -= d;
             }
-            if ((e & kBroke) && !bad && c > dsub[b]) bad = true;      // the reference would have gone on
+            if (!fits || ((e & kBroke) && c > dsub[b])) bad = true;   // closed early, or would have gone on
             w.capa[s] = c;
         }
         if (x.any(bad)) {

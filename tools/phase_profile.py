@@ -30,7 +30,8 @@ from metis_b200.gpu_cluster import GPUCluster  # noqa: E402
 from metis_b200.utils import ModelConfig  # noqa: E402
 from metis_b200.workloads import WORKLOADS, materialize, profile_file_order  # noqa: E402
 
-NAMES = {0: 'fetch+decode', 1: 'begin+strategy', 2: 'P perf', 9: 'R init', 10: 'R forward', 18: 'R seq forward',
+NAMES = {0: 'fetch+decode', 1: 'begin+strategy', 2: 'P perf', 9: 'R init', 10: 'R fwd walk', 19: 'R fwd replay',
+         18: 'R seq forward',
          11: 'R backward', 12: 'R leftovers', 17: 'R middle', 13: 'R vote', 14: 'R cnt+capa', 15: 'R adjust',
          16: 'R part', 20: 'M demand', 21: 'M reweight', 22: 'C stage terms', 23: 'C sums+emit', 24: 'chain advance',
          25: 'drain', 30: 'gate wait'}
