@@ -183,7 +183,8 @@ void metis_set_profile_events(void *before_kernel, void *after_kernel);
 
 /* Bytes of device scratch metis_het_search needs for a shard of `num_plans` plans: the packed tables
  * plus two lists of 16 B per plan (worst case: every plan has a valid strategy); `max_stage` is ignored.
- * metis_het_detail / metis_homo_cost need metis_het_workspace_bytes(problem, 0, 1).
+ * metis_het_detail / metis_het_trace / metis_het_breakdown / metis_homo_cost / metis_homo_breakdown need
+ * metis_het_workspace_bytes(problem, 0, 1).
  * About 36 B per plan in all: a space whose workspace, rows and records do not fit the device (or that has 2^32
  * plans or 4 GiB of rows) is searched in ordinal windows, each a MetisPlanSpace of its own
  * (metis_b200.flatten.plan_windows sizes them with this function). */
@@ -221,6 +222,56 @@ int metis_het_detail(const MetisProblem *problem, const MetisPlanSpace *space, c
  */
 int metis_het_trace(const MetisProblem *problem, const MetisPlanSpace *space, const uint32_t *ordinals, int64_t n,
                     uint64_t *trace, int32_t words_per_plan, void *workspace, int64_t workspace_bytes, void *stream);
+
+/*
+ * Cost breakdown of costed candidates: what HeteroCostEstimator.get_cost adds up (model/cost_estimator.py:235-242) and
+ * the memory headroom of the accepted partition attempt (IntraStagePlan.memory_state, model/load_balancer.py:57-63).
+ */
+typedef struct MetisBreakdown {          /* 64 B per candidate */
+    double terms[6];              /* execution, fb_sync, max parameter update, max dp, pp, batch generate; summed left to
+                                     right they give the record's cost                                            */
+    double min_headroom;          /* min over the stages of memory_state (capacity - demand)                        */
+    int16_t min_stage;            /* its stage, lowest on ties                                                      */
+    int16_t costed_stages;        /* min(InterStagePlan.num_stage, len(device_groups)): the stages get_cost walks (Q1) */
+    int16_t num_stage;            /* len(device_groups); 0 = the pick is not a costed candidate of the space        */
+    int16_t reserved;
+} MetisBreakdown;
+
+/* per-stage fields of metis_het_breakdown's stage_out, in this order */
+#define METIS_BD_PERFORMANCE  0   /* stage compute performance fed to the accepted balancer run                      */
+#define METIS_BD_EXEC_TIME    1   /* stage execution time (lens[s], cost_estimator.py:208-210)                       */
+#define METIS_BD_CAPACITY     2   /* stage memory capacity                                                          */
+#define METIS_BD_DEMAND       3   /* stage memory demand of the accepted attempt                                    */
+#define METIS_BD_STATE        4   /* memory_state = capacity - demand                                               */
+#define METIS_BD_DP           5   /* dp cost                                                                        */
+#define METIS_BD_UPDATE       6   /* parameter update cost                                                          */
+#define METIS_BD_PP           7   /* pp hop cost to the next stage (0 for the last costed stage)                    */
+#define METIS_BD_FIELDS       8
+
+/*
+ * Replays the plans of the listed candidates (one thread per distinct ordinal; each plan's chain runs once however
+ * many of its steps are asked for) and writes their breakdowns.
+ *   picks     [device] n MetisRecord sorted by (ordinal, step); only ordinal and step are read
+ *   out       [device] n MetisBreakdown
+ *   stage_out [device] optional: n x METIS_BD_FIELDS x stage_stride doubles, field-major per pick; NaN past
+ *             num_stage, and in the cost fields (exec time, dp, update, pp) past costed_stages.
+ *             stage_stride >= num_stage of every pick (a pick with more stages gets no stage rows), or NULL
+ *   workspace [device] metis_het_workspace_bytes(problem, 0, 1) bytes
+ */
+int metis_het_breakdown(const MetisProblem *problem, const MetisPlanSpace *space, const MetisRecord *picks, int64_t n,
+                        MetisBreakdown *out, double *stage_out, int32_t stage_stride, void *workspace,
+                        int64_t workspace_bytes, void *stream);
+
+/*
+ * metis_homo_cost with the cost terms and the per-stage memory sums (HomoCostEstimator.get_cost returns them as
+ * stage_memory, model/cost_estimator.py:121-138).
+ *   terms        [device] n x 6 doubles: execution, fb_sync, parameter update, dp, pp, batch generate
+ *   stage_memory [device] n x stage_stride doubles, NaN past pp
+ *   status       [device] n int32: 0 ok, 1 KeyError (plan skipped), 2 oom flag set, 3 pp > stage_stride
+ */
+int metis_homo_breakdown(const MetisProblem *problem, int32_t type_id, const int32_t *plans, int64_t n, double *terms,
+                         double *stage_memory, int32_t stage_stride, int32_t *status, void *workspace,
+                         int64_t workspace_bytes, void *stream);
 
 /*
  * Replaces HomoCostEstimator.get_cost (model/cost_estimator.py:98-138) for n UniformPlans

@@ -220,6 +220,21 @@ class HetSearchResult(Sequence):
             order = order[:k]
         return self.candidates.tuples(order)
 
+    def breakdown(self, idx, per_stage: bool = True):
+        """Cost terms and memory headroom of the candidates at ``idx`` (an int, a slice or an index array of positions
+        in estimate_costs order; ranked positions: ``result.breakdown(result.rank_order[:k])`` after ``ranked()``),
+        replayed on the GPU (metis_het_breakdown).  Returns a search.Breakdown with one row per position asked for;
+        ``per_stage=False`` leaves out the per-stage arrays."""
+        n = len(self)
+        if isinstance(idx, slice):
+            pos = np.arange(n)[idx]
+        else:
+            pos = np.asarray(idx, dtype=np.int64).reshape(-1)
+            pos = np.where(pos < 0, pos + n, pos)
+            if len(pos) and (pos.min() < 0 or pos.max() >= n):
+                raise IndexError('list index out of range')
+        return self.candidates.breakdown(pos, per_stage)
+
     def best(self) -> Optional[Tuple]:
         """argmin (cost, position): the first entry of the ranked list.  The search kernels reduce it on the device
         (het_finalize_kernel: lowest cost, then lowest ordinal, then lowest step), so no sort is needed for it."""
@@ -368,7 +383,7 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     t2 = time.perf_counter()
     # the row blob of the engine is rewritten by the next call: a lazy result keeps its own copy (a few MB, on the GPU)
     cand = search.Candidates(out.records, out.detail, space, seqs, detail_dev=out.detail_dev,
-                             rows_dev=dp.rows_device().clone())
+                             rows_dev=dp.rows_device().clone(), problem=problem)
     # sorted(result, key=cost) is the CALLER's step in the reference (cost_het_cluster.py:76): its permutation is
     # computed by the device sort when ranked() is first asked for; best() needs no sort at all
     result = HetSearchResult(cand, out.rank_order,
@@ -516,8 +531,42 @@ def cost_homo_cluster(args: argparse.Namespace, gpu_cluster, cost_estimator: Hom
                       device_type: Optional[str] = None, device=None) -> List[Tuple[UniformPlan, float]]:
     """cost_homo_cluster.py:21-37 on the GPU: every gbs-matching UniformPlan is costed by
     homo_cost_kernel; plans whose profile key is missing are skipped like ``except KeyError``."""
-    from copy import copy
     from . import search
+    plans, problem, table, type_id = _homo_inputs(args, gpu_cluster, cost_estimator, device_type)
+    cost, status = search.homo_costs(problem, type_id, table, device)
+    return [(p, float(c)) for p, c, s in zip(plans, cost, status) if s != 1]
+
+
+@dataclass
+class HomoBreakdown:
+    """What HomoCostEstimator.get_cost computes besides the cost (model/cost_estimator.py:98-138), for the plans of
+    cost_homo_cluster() in its order.  ``terms[:, k]`` is search.TERM_NAMES[k]; summed left to right they give the
+    plan's cost."""
+    plans: List[UniformPlan]
+    terms: np.ndarray                     # float64 [n, 6]
+    stage_memory: np.ndarray              # float64 [n, largest pp]: sum of the profiled memory of each stage, NaN past pp
+    stage_memory_str: List[List[str]]     # the reference's f'{round(m/1024/1024/1024, 2)}GB' per stage
+    oom: np.ndarray                       # bool [n]: _detect_oom_occurrence
+
+
+def cost_homo_breakdown(args: argparse.Namespace, gpu_cluster, cost_estimator: HomoCostEstimator,
+                        device_type: Optional[str] = None, device=None) -> HomoBreakdown:
+    """The cost terms, per-stage memory and OOM flag of exactly the plans cost_homo_cluster() returns, on the GPU
+    (homo_breakdown_kernel)."""
+    from . import search
+    plans, problem, table, type_id = _homo_inputs(args, gpu_cluster, cost_estimator, device_type)
+    terms, mem, status = search.homo_breakdown(problem, type_id, table, device)
+    keep = status != 1
+    mem = mem[keep]
+    pp = table[keep, 1]
+    strs = [[f'{round(float(m) / 1024 / 1024 / 1024, 2)}GB' for m in row[:k]] for row, k in zip(mem, pp.tolist())]
+    return HomoBreakdown([p for p, k in zip(plans, keep) if k], terms[keep], mem, strs, status[keep] == 2)
+
+
+def _homo_inputs(args, gpu_cluster, cost_estimator: HomoCostEstimator, device_type: Optional[str]):
+    """(gbs-matching UniformPlans, flattened problem, their (dp, pp, tp, mbs, gbs) table, type id) of
+    cost_homo_cluster()."""
+    from copy import copy
     profile_data = cost_estimator.profile_data
     if device_type is None:
         device_type = next(k for k in profile_data if k.startswith('DeviceType.')).split('.', 1)[1]
@@ -536,5 +585,4 @@ def cost_homo_cluster(args: argparse.Namespace, gpu_cluster, cost_estimator: Hom
     if device_type not in problem.type_names:
         raise KeyError(f'DeviceType.{device_type}')
     table = np.array([[p.dp, p.pp, p.tp, p.mbs, p.gbs] for p in plans], dtype=np.int32).reshape(-1, 5)
-    cost, status = search.homo_costs(problem, problem.type_names.index(device_type), table, device)
-    return [(p, float(c)) for p, c, s in zip(plans, cost, status) if s != 1]
+    return plans, problem, table, problem.type_names.index(device_type)

@@ -840,7 +840,8 @@ MB_HD_NOINLINE int partition_data(const Tables &T, int ns, int rank_lo, int coun
 //   void fatal(uint32_t ordinal, int code, uint32_t aux);
 //   void emit(const PlanDesc&, int step, int nrep, double cost, const uint8_t *tpc, const uint16_t *part);
 
-// Optional tap of intermediate values for the verbose transcript (metis_trace.cuh); null in the search kernels.
+// Optional tap of intermediate values for the verbose transcript and the cost breakdown (metis_trace.cuh); null in
+// the search kernels.  homo_cost fills `demand` (per-stage memory sums, cost_estimator.py:121-122) and `cost` only.
 struct TraceTap {
     double *demand;     // [S] stage_memory_demand of the last partition attempt (load_balancer.py:133)
     double *state;      // [S] memory_state of that attempt
@@ -1565,10 +1566,11 @@ MB_HD bool first_task(const Tables &T, Scratch<MAXS, MAXL> &w, Sink &sink, bool 
 
 // ---------------------------------------------------------------------------
 // HomoCostEstimator.get_cost (model/cost_estimator.py:98-138) for one UniformPlan.
-// returns 0 ok, 1 KeyError; *oom = _detect_oom_occurrence
+// returns 0 ok, 1 KeyError; *oom = _detect_oom_occurrence; `tap` (breakdown only) gets the per-stage memory sums
+// and the cost terms
 // ---------------------------------------------------------------------------
 MB_HD int homo_cost(const Tables &T, int type, int dp, int pp, int tp, int mbs, int gbs, double &cost_out,
-                    int &oom) {
+                    int &oom, TraceTap *tap = nullptr) {
     const int L = T.p.num_layers;
     const int per = T.p.devices_per_node;
     int tpc = 0;
@@ -1605,6 +1607,7 @@ MB_HD int homo_cost(const Tables &T, int type, int dp, int pp, int tp, int mbs, 
         if (sp > max_params) max_params = sp;
         const double sm = py_sum_range(T.mem + (size_t)key * T.p.lpad, a, b);
         if (sm > max_mem) max_mem = sm;
+        if (tap) tap->demand[s] = sm;
         if (s == pp - 1) {
             const double v = T.fb_sync[key];
             if (v == 0.0) return 1;
@@ -1635,6 +1638,7 @@ MB_HD int homo_cost(const Tables &T, int type, int dp, int pp, int tp, int mbs, 
     const double dpc = (double)(2 * (dp - 1)) / ((double)dp * (bw * 1048576.0)) * max_params;
     const double bg = T.p.batch_generator * (double)num_mbs;
     cost_out = exec + fb_sync + upd + dpc + pp_cost + bg;
+    if (tap) { tap->cost[0] = exec; tap->cost[1] = fb_sync; tap->cost[2] = upd; tap->cost[3] = dpc; tap->cost[4] = pp_cost; }
     return 0;
 }
 

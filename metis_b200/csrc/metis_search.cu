@@ -19,7 +19,9 @@
 //   het_finalize_kernel   grid argmin over the per-block bests, counters -> summary
 //   het_detail_kernel     replays chosen (ordinal, step) candidates to materialise strategies/partition
 //   het_trace_kernel      replays plans and records what the reference prints (metis_trace.cuh)
+//   het_breakdown_kernel  replays chosen candidates, one thread per plan, for their cost terms and memory headroom
 //   homo_cost_kernel      a17: one thread per UniformPlan
+//   homo_breakdown_kernel the same with the cost terms and per-stage memory
 //   layer_balance_kernel  a10 alone, for unit parity
 //   (rank_records_kernel, the stable record sort, lives in metis_rank.cu)
 //
@@ -697,6 +699,35 @@ het_trace_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
     out.finish();
 }
 
+// cost breakdown: the first thread of every run of equal ordinals replays that plan once and writes each of its picks
+// (metis_trace.cuh, BreakdownEvaluator)
+__global__ void __launch_bounds__(kThreads)
+het_breakdown_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ MetisPlanSpace sp,
+                     const __grid_constant__ BlobLayout lay, const uint8_t *__restrict__ blob,
+                     const MetisRecord *__restrict__ picks, long long n, MetisBreakdown *out, double *stage_out,
+                     int stride) {
+    const Tables T = make_tables(p, lay, blob);
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n || (i > 0 && picks[i - 1].ordinal == picks[i].ordinal)) return;
+    long long end = i + 1;
+    while (end < n && picks[end].ordinal == picks[i].ordinal) ++end;
+    Scratch<kMaxS, kMaxL> w;
+    BreakdownEvaluator<kMaxS, kMaxL> ev(T, w, picks, i, end, out, stage_out, stride);
+    for (long long k = i; k < end; ++k) ev.clear(k);
+    PlanDesc pd;
+    if (decode_plan(sp, picks[i].ordinal, pd)) ev.replay(pd);
+}
+
+__global__ void __launch_bounds__(kThreads)
+homo_breakdown_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ BlobLayout lay,
+                      const uint8_t *__restrict__ blob, int type_id, const int32_t *__restrict__ plans, long long n,
+                      double *terms, double *stage_memory, int stride, int32_t *status) {
+    const Tables T = make_tables(p, lay, blob);
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    status[i] = homo_breakdown(T, type_id, plans + i * 5, terms + i * 6, stage_memory + i * stride, stride);
+}
+
 __global__ void __launch_bounds__(kThreads)
 homo_cost_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ BlobLayout lay,
                  const uint8_t *__restrict__ blob, int type_id, const int32_t *__restrict__ plans, long long n,
@@ -1079,6 +1110,52 @@ int metis_het_trace(const MetisProblem *problem, const MetisPlanSpace *space, co
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "het_trace_kernel");
+    return METIS_OK;
+}
+
+int metis_het_breakdown(const MetisProblem *problem, const MetisPlanSpace *space, const MetisRecord *picks, int64_t n,
+                        MetisBreakdown *out, double *stage_out, int32_t stage_stride, void *workspace,
+                        int64_t workspace_bytes, void *stream_) {
+    int rc = check_problem(problem);
+    if (rc) return rc;
+    if (!space || (n > 0 && (!picks || !out)) || !workspace) return arg_fail("NULL argument");
+    if (n < 0) return arg_fail("negative number of picks");
+    if (stage_out && (stage_stride < 1 || stage_stride > METIS_MAX_STAGES)) return arg_fail("stage_stride out of range");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const BlobLayout lay = make_layout(*problem);
+    if (workspace_bytes < 256 + kFixedWs + (int64_t)align16(lay.total)) return METIS_E_CAPACITY;
+    const Workspace ws = carve(workspace, lay);
+    pack_tables_kernel<<<8, 256, 0, stream>>>(*problem, lay, ws.blob);
+    if (n > 0) {
+        const unsigned nb = (unsigned)((n + kThreads - 1) / kThreads);
+        het_breakdown_kernel<<<nb, kThreads, 0, stream>>>(*problem, *space, lay, ws.blob, picks, n, out, stage_out,
+                                                          stage_stride);
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "het_breakdown_kernel");
+    return METIS_OK;
+}
+
+int metis_homo_breakdown(const MetisProblem *problem, int32_t type_id, const int32_t *plans, int64_t n, double *terms,
+                         double *stage_memory, int32_t stage_stride, int32_t *status, void *workspace,
+                         int64_t workspace_bytes, void *stream_) {
+    int rc = check_problem(problem);
+    if (rc) return rc;
+    if (!plans || !terms || !stage_memory || !status || !workspace) return arg_fail("NULL argument");
+    if (type_id < 0 || type_id >= problem->num_types) return arg_fail("type_id out of range");
+    if (stage_stride < 1) return arg_fail("stage_stride out of range");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const BlobLayout lay = make_layout(*problem);
+    if (workspace_bytes < 256 + kFixedWs + (int64_t)align16(lay.total)) return METIS_E_CAPACITY;
+    const Workspace ws = carve(workspace, lay);
+    pack_tables_kernel<<<8, 256, 0, stream>>>(*problem, lay, ws.blob);
+    if (n > 0) {
+        const unsigned nb = (unsigned)((n + kThreads - 1) / kThreads);
+        homo_breakdown_kernel<<<nb, kThreads, 0, stream>>>(*problem, lay, ws.blob, type_id, plans, n, terms, stage_memory,
+                                                           stage_stride, status);
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "homo_breakdown_kernel");
     return METIS_OK;
 }
 

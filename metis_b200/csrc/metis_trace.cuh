@@ -4,6 +4,7 @@
 // state, the re-weighted performance, the cost terms and which KeyError skipped a candidate.  One thread per plan
 // (the sequential PlanEvaluator of metis_eval.cuh, unchanged arithmetic); the host formats the lines
 // (metis_b200/verbose.py).  Debug path of the drop-in CLI (METIS_VERBOSE=1), never used by a search.
+// Also the cost breakdown of chosen candidates (BreakdownEvaluator, homo_breakdown): the same tap, structured output.
 //
 // Event stream per plan: 64-bit words.  A header word  tag | n << 8 | aux << 32  is followed by its payload.
 #pragma once
@@ -209,5 +210,110 @@ struct TraceEvaluator : PlanEvaluator<MAXS, MAXL, Serial, false> {
         }
     }
 };
+
+// ---------------------------------------------------------------------------
+// Cost breakdown of costed candidates (metis_het_breakdown).  PlanEvaluator::run replays one plan's chain once, up to
+// the last requested step, with this evaluator as its own sink.  The tap holds the memory demand and state of the
+// last partition attempt and the five printed cost terms; at an emitted step that attempt is the accepted one, and
+// the scratch still holds the performance fed to its balancer run, the strategies and the partition.  The per-stage
+// cost values come from the same stage_time / stage_terms members get_cost adds up, so they are the same bits.
+// ---------------------------------------------------------------------------
+template <int MAXS, int MAXL>
+struct BreakdownEvaluator : PlanEvaluator<MAXS, MAXL, Serial, false> {
+    using Base = PlanEvaluator<MAXS, MAXL, Serial, false>;
+    using Base::T; using Base::w;
+    double tap_demand[MAXS], tap_state[MAXS];
+    TraceTap tap_store;
+    const MetisRecord *picks;     // picks[at, end): the requested steps of this plan, ascending
+    int64_t at, end;
+    MetisBreakdown *out;
+    double *stage_out;            // null, or METIS_BD_FIELDS x stride doubles per pick
+    int stride;
+
+    MB_HD BreakdownEvaluator(const Tables &t, Scratch<MAXS, MAXL> &s, const MetisRecord *p, int64_t first, int64_t last,
+                             MetisBreakdown *o, double *so, int st)
+        : Base(t, s), picks(p), at(first), end(last), out(o), stage_out(so), stride(st) {
+        tap_store.demand = tap_demand;
+        tap_store.state = tap_state;
+        this->tap = &tap_store;
+    }
+
+    // sink interface of PlanEvaluator::run
+    MB_HD void phase(int) {}
+    MB_HD void partition_call() {}
+    MB_HD void balancer_run() {}
+    MB_HD void keyerror() {}
+    MB_HD void fatal(uint32_t, int, uint32_t) {}
+    MB_HD void emit(const PlanDesc &pd, int step, int, double, const uint8_t *, const uint16_t *) {
+        while (at < end && (int)picks[at].step < step) ++at;  // a step the chain never yields keeps its empty row
+        for (; at < end && (int)picks[at].step == step; ++at) write(pd, at);
+    }
+
+    // every requested row empty first: num_stage 0, NaN everywhere
+    MB_HD void clear(int64_t i) {
+        MetisBreakdown b;
+        for (int k = 0; k < 6; ++k) b.terms[k] = NAN;
+        b.min_headroom = NAN;
+        b.min_stage = -1; b.costed_stages = 0; b.num_stage = 0; b.reserved = 0;
+        out[i] = b;
+        if (stage_out)
+            for (int k = 0; k < METIS_BD_FIELDS * stride; ++k) stage_out[(size_t)i * METIS_BD_FIELDS * stride + k] = NAN;
+    }
+
+    MB_HD void write(const PlanDesc &pd, int64_t i) {
+        const int S = pd.S, nstage = pd.label < S ? pd.label : S;
+        MetisBreakdown b;
+        for (int k = 0; k < 5; ++k) b.terms[k] = tap_store.cost[k];
+        b.terms[5] = T.p.batch_generator * (double)pd.batches;   // get_cost's batch generate term
+        int lo = 0;
+        for (int s = 1; s < S; ++s)
+            if (tap_state[s] < tap_state[lo]) lo = s;
+        b.min_headroom = tap_state[lo];
+        b.min_stage = (int16_t)lo;
+        b.costed_stages = (int16_t)nstage;
+        b.num_stage = (int16_t)S;
+        b.reserved = 0;
+        out[i] = b;
+        if (!stage_out || S > stride) return;
+        double *f = stage_out + (size_t)i * METIS_BD_FIELDS * stride;
+        for (int s = 0; s < S; ++s) {
+            const int a = this->rank_start(s);
+            f[METIS_BD_PERFORMANCE * stride + s] = w.perf[s];
+            f[METIS_BD_CAPACITY * stride + s] = this->memory_capacity(a, a + this->group(s));
+            f[METIS_BD_DEMAND * stride + s] = tap_demand[s];
+            f[METIS_BD_STATE * stride + s] = tap_state[s];
+            if (s >= nstage) continue;
+            double len, pp, dpc, upd;
+            this->stage_time(s, len);
+            this->stage_terms(s, nstage, pp, dpc, upd);
+            f[METIS_BD_EXEC_TIME * stride + s] = len;
+            f[METIS_BD_DP * stride + s] = dpc;
+            f[METIS_BD_UPDATE * stride + s] = upd;
+            f[METIS_BD_PP * stride + s] = pp;
+        }
+    }
+
+    // the requested steps of one plan (pd = the plan of picks[at])
+    MB_HD void replay(const PlanDesc &pd) {
+        this->run(pd, *this, (int)picks[end - 1].step);
+    }
+};
+
+// HomoCostEstimator.get_cost of one UniformPlan (dp, pp, tp, mbs, gbs) with its breakdown (metis_homo_breakdown):
+// terms[6], the per-stage memory sums in mem[0, stride) (NaN past pp); returns the status word of metis_homo_breakdown
+MB_HD int homo_breakdown(const Tables &T, int type, const int32_t *q, double *terms, double *mem, int stride) {
+    for (int k = 0; k < 6; ++k) terms[k] = NAN;
+    for (int s = 0; s < stride; ++s) mem[s] = NAN;
+    if (q[1] > stride) return 3;
+    TraceTap tap;
+    tap.demand = mem;
+    tap.state = nullptr;
+    double c = 0.0;
+    int oom = 0;
+    if (homo_cost(T, type, q[0], q[1], q[2], q[3], q[4], c, oom, &tap)) return 1;
+    for (int k = 0; k < 5; ++k) terms[k] = tap.cost[k];
+    terms[5] = T.p.batch_generator * (double)(q[4] / q[3] / q[0]);   // the batch generate term of homo_cost
+    return oom ? 2 : 0;
+}
 
 }  // namespace metis

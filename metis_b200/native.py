@@ -83,9 +83,13 @@ BLOCK_DTYPE = [('first_ordinal', '<i8'), ('rows_offset', '<i8'), ('num_rows', '<
 COMP_DTYPE = [('row_offset', '<i8'), ('pool_offset', '<u4'), ('stages', '<u2'), ('num_groups', '<u2'),
               ('first_row', '<u4'), ('num_rows', '<u4')]
 RANGE_DTYPE = [('stages', '<i4'), ('reserved', '<i4'), ('first_row', '<i8'), ('end_row', '<i8')]   # MetisRowRange
+BREAKDOWN_DTYPE = [('terms', '<f8', (6,)), ('min_headroom', '<f8'), ('min_stage', '<i2'), ('costed_stages', '<i2'),
+                   ('num_stage', '<i2'), ('reserved', '<i2')]                                     # MetisBreakdown
+BD_FIELDS = 8                                  # METIS_BD_FIELDS: per-stage fields of metis_het_breakdown's stage_out
 
 SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 'metis_het_workspace_bytes', 'metis_het_search',
-           'metis_het_detail', 'metis_het_trace', 'metis_homo_cost', 'metis_layer_balance', 'metis_enum_device_groups',
+           'metis_het_detail', 'metis_het_trace', 'metis_het_breakdown', 'metis_homo_cost',
+           'metis_homo_breakdown', 'metis_layer_balance', 'metis_enum_device_groups',
            'metis_enum_device_group_tables', 'metis_sort_workspace_bytes', 'metis_sort_records',
            'metis_enum_compositions', 'metis_generate_rows', 'metis_list_workspace_bytes', 'metis_list_stages',
            'metis_list_window']
@@ -124,6 +128,12 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_het_trace.restype = C.c_int
     lib.metis_het_trace.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.c_void_p, C.c_int64,
                                     C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.metis_het_breakdown.restype = C.c_int
+    lib.metis_het_breakdown.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.c_void_p, C.c_int64,
+                                        C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.metis_homo_breakdown.restype = C.c_int
+    lib.metis_homo_breakdown.argtypes = [C.POINTER(MetisProblem), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
+                                         C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     lib.metis_homo_cost.restype = C.c_int
     lib.metis_homo_cost.argtypes = [C.POINTER(MetisProblem), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

@@ -371,9 +371,10 @@ class Candidates:
 
     def __init__(self, records: np.ndarray, detail: Optional[np.ndarray], space: flatten.FlatPlanSpace,
                  node_sequences: Sequence[Tuple], detail_dev: Optional[torch.Tensor] = None,
-                 rows_dev: Optional[torch.Tensor] = None):
+                 rows_dev: Optional[torch.Tensor] = None, problem: Optional[flatten.FlatProblem] = None):
         self.records = records
         self.space = space
+        self.problem = problem                # the tables breakdown() replays the candidates on
         self.node_sequences = [tuple(s) for s in node_sequences]
         self._detail = detail
         self._detail_dev = detail_dev
@@ -417,6 +418,28 @@ class Candidates:
         """Position of the candidate (ordinal, step), or None: bisection over the (ordinal, step)-sorted records."""
         return _bisect_records(self.records, 0, len(self.records), int(ordinal), int(step))
 
+    def breakdown(self, idx, per_stage: bool = True) -> Breakdown:
+        """Cost terms and memory headroom of the candidates ``idx`` (metis_het_breakdown).  The problem tables and plan
+        space descriptors are uploaded from this object's own copies, so a later search cannot change what is
+        replayed."""
+        if self.problem is None:
+            raise ValueError('these candidates were built without their problem tables: no breakdown')
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        dev = self._rows_dev.device if self._rows_dev is not None else _require_cuda(None)
+        lib = native.load_library()
+        with torch.cuda.device(dev):
+            tens = {k: torch.from_numpy(np.ascontiguousarray(v).view(np.uint8).reshape(-1).copy()).to(dev)
+                    for k, v in self.problem.arrays.items()}
+            for k in ('blocks', 'batches'):
+                tens[k] = torch.from_numpy(np.ascontiguousarray(getattr(self.space, k)).view(np.uint8).reshape(-1)
+                                           .copy()).to(dev)
+            tens['rows'] = self._rows_dev if self._rows_dev is not None else torch.from_numpy(self._rows).to(dev)
+            p = self.problem.as_struct(lambda n: tens[n].data_ptr())
+            sp = self.space.as_struct(lambda n: tens[n].data_ptr())
+            ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=dev)
+            raw, stages = het_breakdown(lib, p, sp, ws, self.records[idx], dev, per_stage)
+        return Breakdown.from_raw(raw, stages)
+
     def detail_rows(self, idx: np.ndarray) -> np.ndarray:
         if self._detail is None:
             if self._detail_dev is None:
@@ -449,6 +472,81 @@ class Candidates:
             out.append((self.node_sequences[int(col['ns_idx'][k])], groups, list(zip(dp, tp)), int(col['batches'][k]),
                         part, int(col['num_repartition'][k]), float(cost[k])))
         return out
+
+
+TERM_NAMES = ('execution', 'fb_sync', 'parameter_update', 'dp', 'pp', 'batch_generate')
+# the per-stage fields of metis_het_breakdown, in the order of METIS_BD_*
+STAGE_FIELDS = ('performance', 'stage_time', 'memory_capacity', 'memory_demand', 'memory_state', 'dp_cost',
+                'update_cost', 'pp_cost')
+
+
+@dataclass
+class Breakdown:
+    """Cost terms and memory headroom of chosen candidates (metis_het_breakdown), one row per candidate in the order
+    asked for.  ``terms[:, k]`` is TERM_NAMES[k] (model/cost_estimator.py:235-242): summed left to right they give the
+    candidate's cost.  The per-stage arrays ([n, largest num_stage], NaN past a candidate's stages) hold the accepted
+    partition attempt's values (model/load_balancer.py:57-63); the cost fields (stage_time, dp_cost, update_cost,
+    pp_cost) cover the ``costed_stages`` stages get_cost walks and are NaN after them (quirk Q1).  They are None when
+    the breakdown was asked for without per-stage values."""
+    terms: np.ndarray                     # float64 [n, 6]
+    min_headroom: np.ndarray              # float64 [n]: min over the stages of memory_state
+    min_headroom_stage: np.ndarray        # int [n]: its stage, lowest on ties
+    num_stage: np.ndarray                 # int [n]: len(device_groups)
+    costed_stages: np.ndarray             # int [n]: min(InterStagePlan.num_stage, len(device_groups))
+    performance: Optional[np.ndarray] = None
+    stage_time: Optional[np.ndarray] = None
+    memory_capacity: Optional[np.ndarray] = None
+    memory_demand: Optional[np.ndarray] = None
+    memory_state: Optional[np.ndarray] = None
+    dp_cost: Optional[np.ndarray] = None
+    update_cost: Optional[np.ndarray] = None
+    pp_cost: Optional[np.ndarray] = None
+
+    def __len__(self) -> int:
+        return len(self.terms)
+
+    @classmethod
+    def from_raw(cls, raw: np.ndarray, stages: Optional[np.ndarray]) -> 'Breakdown':
+        """MetisBreakdown rows (+ [n, METIS_BD_FIELDS, width] per-stage values) -> Breakdown."""
+        per = {} if stages is None else {f: np.ascontiguousarray(stages[:, k, :]) for k, f in enumerate(STAGE_FIELDS)}
+        return cls(np.array(raw['terms']), np.array(raw['min_headroom']), raw['min_stage'].astype(np.int64),
+                   raw['num_stage'].astype(np.int64), raw['costed_stages'].astype(np.int64), **per)
+
+
+_BREAKDOWN_CHUNK = 1 << 16                 # picks per launch: bounds the per-stage buffers of one call
+
+
+def het_breakdown(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.ndarray, device,
+                  per_stage: bool = True, width: Optional[int] = None) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+    """metis_het_breakdown of ``records`` (any order) on the problem / space bound in ``p_struct`` / ``s_struct``:
+    the picks are sorted by (ordinal, step), so that each plan is replayed once, and the rows scattered back to the
+    order given.  Returns (MetisBreakdown rows, per-stage values [n, METIS_BD_FIELDS, width] or None)."""
+    n = len(records)
+    order = np.lexsort((records['step'], records['ordinal']))
+    picks = np.ascontiguousarray(records[order])
+    width = int(width or (int(picks['num_stage'].max()) if n else 1))
+    raw = np.zeros(n, dtype=native.BREAKDOWN_DTYPE)
+    stages = np.full((n, native.BD_FIELDS, width), np.nan) if per_stage else None
+    with torch.cuda.device(device):
+        s = torch.cuda.current_stream(device)
+        for lo in range(0, n, _BREAKDOWN_CHUNK):
+            hi = min(n, lo + _BREAKDOWN_CHUNK)
+            d_picks = torch.from_numpy(picks[lo:hi].view(np.uint8).reshape(-1).copy()).to(device)
+            d_out = torch.empty((hi - lo) * raw.itemsize, dtype=torch.uint8, device=device)
+            d_st = torch.empty((hi - lo) * native.BD_FIELDS * width, dtype=torch.float64, device=device) \
+                if per_stage else None
+            rc = lib.metis_het_breakdown(C.byref(p_struct), C.byref(s_struct), C.c_void_p(d_picks.data_ptr()),
+                                         C.c_int64(hi - lo), C.c_void_p(d_out.data_ptr()),
+                                         C.c_void_p(d_st.data_ptr() if per_stage else 0), C.c_int32(width),
+                                         C.c_void_p(workspace.data_ptr()), C.c_int64(workspace.numel()),
+                                         C.c_void_p(s.cuda_stream))
+            native.check(rc, 'metis_het_breakdown')
+            raw[lo:hi] = d_out.cpu().numpy().view(native.BREAKDOWN_DTYPE)
+            if per_stage:
+                stages[lo:hi] = d_st.cpu().numpy().reshape(hi - lo, native.BD_FIELDS, width)
+    back = np.empty(n, dtype=np.int64)
+    back[order] = np.arange(n)
+    return raw[back], (stages[back] if per_stage else None)
 
 
 def materialize(records: np.ndarray, detail: np.ndarray, space: flatten.FlatPlanSpace,
@@ -711,6 +809,23 @@ class WindowedCandidates:
                 out[k] = t
         return out
 
+    def breakdown(self, idx, per_stage: bool = True) -> Breakdown:
+        """Cost terms and memory headroom of the candidates ``idx``, window by window like tuples()."""
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        width = max(int(self.records['num_stage'][idx].max()), 1) if len(idx) else 1
+        raw = np.zeros(len(idx), dtype=native.BREAKDOWN_DTYPE)
+        stages = np.full((len(idx), native.BD_FIELDS, width), np.nan) if per_stage else None
+        win = np.searchsorted(self.firsts, idx, side='right') - 1
+        for w in np.unique(win).tolist():
+            at = np.nonzero(win == w)[0]
+            dp = self._load(w)
+            r, st = het_breakdown(dp.lib, dp.p_struct, dp.s_struct, self.searcher.workspace, self.records[idx[at]],
+                                  dp.device, per_stage, width)
+            raw[at] = r
+            if per_stage:
+                stages[at] = st
+        return Breakdown.from_raw(raw, stages)
+
 
 # ---------------------------------------------------------------------------------------------
 # multi-GPU: shard by plan ordinal, one collective at the end (SURVEY.md section 8e)
@@ -876,6 +991,34 @@ def homo_costs(problem: flatten.FlatProblem, type_id: int, plans: np.ndarray, de
         native.check(rc, 'metis_homo_cost')
         s.synchronize()
         return cost[:n].cpu().numpy(), status[:n].cpu().numpy()
+
+
+def homo_breakdown(problem: flatten.FlatProblem, type_id: int, plans: np.ndarray, device=None
+                   ) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """metis_homo_breakdown for every row (dp, pp, tp, mbs, gbs) of ``plans``: (terms [n, 6], per-stage memory
+    [n, largest pp] NaN-padded, status: 0 ok, 1 KeyError, 2 oom)."""
+    dev = _require_cuda(device)
+    lib = native.load_library()
+    plans = np.ascontiguousarray(plans, dtype=np.int32).reshape(-1, 5)
+    n = len(plans)
+    width = max(int(plans[:, 1].max()) if n else 1, 1)
+    with torch.cuda.device(dev):
+        tens = {k: torch.from_numpy(np.ascontiguousarray(v).view(np.uint8).reshape(-1).copy()).to(dev)
+                for k, v in problem.arrays.items()}
+        p = problem.as_struct(lambda k: tens[k].data_ptr())
+        ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=dev)
+        d_plans = torch.from_numpy(plans.reshape(-1)).to(dev)
+        terms = torch.empty((max(n, 1), 6), dtype=torch.float64, device=dev)
+        mem = torch.empty((max(n, 1), width), dtype=torch.float64, device=dev)
+        status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        s = torch.cuda.current_stream(dev)
+        rc = lib.metis_homo_breakdown(C.byref(p), C.c_int32(type_id), C.c_void_p(d_plans.data_ptr()), C.c_int64(n),
+                                      C.c_void_p(terms.data_ptr()), C.c_void_p(mem.data_ptr()), C.c_int32(width),
+                                      C.c_void_p(status.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_int64(ws.numel()),
+                                      C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_homo_breakdown')
+        s.synchronize()
+        return terms[:n].cpu().numpy(), mem[:n].cpu().numpy(), status[:n].cpu().numpy()
 
 
 def layer_balance(capa_rows: Sequence[Sequence[float]], lc: Sequence[float], num_layers: int, device=None
