@@ -205,6 +205,17 @@ int metis_het_search(const MetisProblem *problem, const MetisPlanSpace *space, c
                      void *workspace, int64_t workspace_bytes, MetisSearchSummary *summary, void *stream);
 
 /*
+ * metis_het_search that also writes each record's memory headroom: headroom[i] = min over all num_stage stages of
+ * memory_state (capacity - demand, model/load_balancer.py:57-63) of the partition attempt that record i accepted,
+ * the value MetisBreakdown.min_headroom reports for it.
+ *   headroom [device] capacity doubles aligned with records, or NULL (then exactly metis_het_search)
+ */
+int metis_het_search_headroom(const MetisProblem *problem, const MetisPlanSpace *space, const MetisShard *shard,
+                              MetisRecord *records, int64_t capacity, uint8_t *detail, int32_t detail_stride,
+                              double *headroom, void *workspace, int64_t workspace_bytes, MetisSearchSummary *summary,
+                              void *stream);
+
+/*
  * Re-evaluates the listed (ordinal, step) candidates and writes their strategies and
  * partition (same layout as `detail` above).  Used to materialise the winner / a ranked slice.
  *   picks [device] n MetisRecord (only ordinal and step are read)
@@ -311,6 +322,28 @@ int metis_layer_balance(const double *capa, const int32_t *num_stage, int64_t n,
 int64_t metis_sort_workspace_bytes(int64_t n);
 int metis_sort_records(MetisRecord *records, int64_t n, int32_t mode, uint32_t *perm_out, void *workspace,
                        int64_t workspace_bytes, void *stream);
+
+/*
+ * Headroom-constrained views of the ranked list (metis_select.cu).  Inputs, all on the device:
+ *   records  n records in estimate_costs order (only the cost is read)
+ *   headroom n doubles aligned with records (metis_het_search_headroom), no NaN
+ *   rank     n uint32: the perm_out of metis_sort_records(METIS_SORT_BY_COST_STABLE) on those records, i.e. the
+ *            ranked list sorted(estimate_costs, key=cost) as positions in estimate_costs order
+ *   workspace [device] metis_headroom_workspace_bytes(n) bytes
+ *   count    [host] written asynchronously (use pinned memory)
+ *
+ * metis_headroom_select: the first k entries of the ranked list whose headroom is >= min_headroom (finite), in ranked
+ *   order, as positions into out [device, k uint32]; *count = how many of the n qualify.
+ * metis_headroom_front: the cost / headroom Pareto front.  A candidate is on it iff no other one has cost <= and
+ *   headroom >= with one of the two strict; of several with equal (cost, headroom) only the first in estimate_costs
+ *   order is kept.  out [device, n uint32] gets the front's positions by ascending cost (headroom then strictly
+ *   increases); *count = the front's length.
+ */
+int64_t metis_headroom_workspace_bytes(int64_t n);
+int metis_headroom_select(const double *headroom, const uint32_t *rank, int64_t n, double min_headroom, int64_t k,
+                          uint32_t *out, uint64_t *count, void *workspace, int64_t workspace_bytes, void *stream);
+int metis_headroom_front(const MetisRecord *records, const double *headroom, const uint32_t *rank, int64_t n,
+                         uint32_t *out, uint64_t *count, void *workspace, int64_t workspace_bytes, void *stream);
 
 /*
  * Host-side enumeration of gen_dgroups_for_stages_with_variance (search_space/device_group.py:93-107)

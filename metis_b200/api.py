@@ -172,6 +172,10 @@ class HetSearchResult(Sequence):
     def __init__(self, candidates, rank_order: Optional[np.ndarray], summary: Dict[str, int],
                  timings: Optional[Dict[str, float]] = None, ranker=None, best_key: Optional[Tuple[int, int]] = None):
         self.candidates = candidates
+        # fp64 memory headroom of every candidate in estimate_costs order: the smallest memory_state (capacity - demand,
+        # MB) over the stages of its accepted partition attempt; None unless searched with headroom=True
+        self.headroom = getattr(candidates, 'headroom', None)
+        self._headroom_index = None
         self.rank_order = rank_order          # permutation of sorted(..., key=cost); computed on first use (``ranker``)
         self.summary = summary
         self.timings = timings or {}
@@ -209,16 +213,46 @@ class HetSearchResult(Sequence):
         """fp64 cost of every candidate, estimate_costs order (no tuples built)."""
         return self.candidates.cost
 
-    def ranked(self, k: Optional[int] = None) -> List[Tuple]:
-        """The first ``k`` (default: all) entries of ``sorted(result, key=lambda kv: kv[6])``."""
-        if self.rank_order is None:
-            self.rank_order = self._ranker() if self._ranker is not None \
-                else np.argsort(self.candidates.cost, kind='stable')
-            self._ranker = None
+    def ranked(self, k: Optional[int] = None, min_headroom: Optional[float] = None) -> List[Tuple]:
+        """The first ``k`` (default: all) entries of ``sorted(result, key=lambda kv: kv[6])``.  With ``min_headroom``
+        (MB, finite; needs ``headroom=True``): the first ``k`` of those whose headroom is at least that, in ranked
+        order (metis_headroom_select on the GPU); ``k`` must then be >= 0 (a count, not a slice bound)."""
+        if min_headroom is not None:
+            from . import search
+            x = search.check_threshold(min_headroom)
+            if k is not None and int(k) < 0:
+                raise ValueError(f'k must be >= 0 with min_headroom, not {k}')
+            pos, _total = self._index().select(x, k)
+            return self.candidates.tuples(pos)
+        self._rank()
         order = self.rank_order
         if k is not None:
             order = order[:k]
         return self.candidates.tuples(order)
+
+    def _rank(self) -> np.ndarray:
+        if self.rank_order is None:
+            self.rank_order = self._ranker() if self._ranker is not None \
+                else np.argsort(self.candidates.cost, kind='stable')
+            self._ranker = None
+        return self.rank_order
+
+    def _index(self):
+        if self.headroom is None:
+            raise ValueError('this result has no headroom: call cost_het_cluster(..., headroom=True)')
+        if self._headroom_index is None:
+            from . import search
+            self._headroom_index = search.HeadroomIndex(self.candidates.records, self.headroom, self._rank(),
+                                                        getattr(self.candidates, 'device', None))
+        return self._headroom_index
+
+    def pareto(self) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The cost / headroom Pareto front (needs ``headroom=True``): (positions in estimate_costs order, their costs,
+        their headrooms), by ascending cost, headroom strictly increasing.  A candidate is on the front iff no other
+        one has cost <= and headroom >= with one of the two strict; of equal (cost, headroom) pairs only the first in
+        estimate_costs order is kept.  Computed by metis_headroom_front on the GPU."""
+        pos = self._index().front()
+        return pos, self.costs[pos], self.headroom[pos]
 
     def breakdown(self, idx, per_stage: bool = True):
         """Cost terms and memory headroom of the candidates at ``idx`` (an int, a slice or an index array of positions
@@ -312,7 +346,7 @@ def release_engines() -> None:
 def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, model_config: ModelConfig,
                      cost_estimator: HeteroCostEstimator, layer_load_balancer: LayerLoadBalancer,
                      node_sequences: Optional[Sequence[Sequence]] = None, device=None,
-                     corrected: Sequence[str] = ()) -> HetSearchResult:
+                     corrected: Sequence[str] = (), headroom: bool = False) -> HetSearchResult:
     """cost_het_cluster.py:21-50 on the GPU.  Returns the same sequence of
     (node_sequence, device_groups, strategies, batches, layer_partition, num_repartition, cost) in the
     same order (see HetSearchResult).  With torch.distributed initialised the plans are sharded over the ranks and
@@ -324,7 +358,11 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     layer to the stage holding most of its seven sub-layers so that none is dropped (load_balancer.py:293-296), 'Q6'
     takes a stage's memory demand from the profile of its own device type (load_balancer.py:41-52 uses the first
     type of the node sequence and, for mixed stages, sums a whole-cluster split).  Results of a corrected search are
-    NOT the reference's; ``result.summary['corrected']`` records what was applied."""
+    NOT the reference's; ``result.summary['corrected']`` records what was applied.
+
+    ``headroom=True``: the search kernels also write every candidate's memory headroom (``result.headroom``), which
+    ``result.ranked(k, min_headroom=...)`` and ``result.pareto()`` need; ``timings['headroom_s']`` is the host time spent
+    ordering and copying it."""
     unknown = set(corrected) - {'Q1', 'Q2', 'Q5', 'Q6'}
     if unknown:
         raise ValueError(f'unknown corrections {sorted(unknown)}: choose from Q1, Q2, Q5, Q6')
@@ -349,11 +387,14 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
             space, windows = windows[0].space, None
     t1 = time.perf_counter()
     if windows is not None:
-        result = _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1)
+        result = _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1, headroom)
         result.summary['listing'] = 'host' if listing is None else 'device'
         return result
     stride = 3 * int(space.blocks['num_stage'].max()) + 1
     dp, searcher = _engine(problem, space, dev, rank, world, stride)
+    searcher.want_headroom = headroom
+    if not headroom:
+        searcher.headroom = None
     dp.upload()
     failure = None
     out = best = None
@@ -383,7 +424,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     t2 = time.perf_counter()
     # the row blob of the engine is rewritten by the next call: a lazy result keeps its own copy (a few MB, on the GPU)
     cand = search.Candidates(out.records, out.detail, space, seqs, detail_dev=out.detail_dev,
-                             rows_dev=dp.rows_device().clone(), problem=problem)
+                             rows_dev=dp.rows_device().clone(), problem=problem,
+                             headroom=np.array(out.headroom) if headroom else None)
     # sorted(result, key=cost) is the CALLER's step in the reference (cost_het_cluster.py:76): its permutation is
     # computed by the device sort when ranked() is first asked for; best() needs no sort at all
     result = HetSearchResult(cand, out.rank_order,
@@ -393,6 +435,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
                              best_key=(best[1], best[2]) if best else None)
     result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
                       'decode_columns_s': time.perf_counter() - t2}
+    if headroom:
+        result.timings['headroom_s'] = out.headroom_s
     return result
 
 
@@ -489,13 +533,13 @@ def _het_windows(problem, space, dev, rank: int, world: int, num_recs: Optional[
 
 
 def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int, dist, corrected, t0: float,
-                      t1: float) -> HetSearchResult:
+                      t1: float, headroom: bool = False) -> HetSearchResult:
     """cost_het_cluster() for a space larger than one search: flatten.plan_windows' windows, searched in ordinal order
     (search.search_windows), merged on the host; the result keeps the records only (search.WindowedCandidates)."""
     from . import search
     failure = merged = searcher = None
     try:
-        merged, _dp, searcher = search.search_windows(problem, windows, dev, rank, world)
+        merged, _dp, searcher = search.search_windows(problem, windows, dev, rank, world, headroom=headroom)
     except Exception as exc:                                  # noqa: BLE001 - re-raised below on every rank
         if not dist:
             raise
@@ -516,7 +560,8 @@ def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int,
     if summary['fatal_ordinal'] != 2 ** 64 - 1:
         search.raise_fatal(summary, problem)                  # the reference dies at that plan (quirk Q8)
     t2 = time.perf_counter()
-    cand = search.WindowedCandidates(merged.records, merged.bases, merged.firsts, windows, problem, seqs, searcher)
+    cand = search.WindowedCandidates(merged.records, merged.bases, merged.firsts, windows, problem, seqs, searcher,
+                                     headroom=merged.headroom)
     result = HetSearchResult(cand, None, dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)),
                                               num_windows=len(windows)),
                              best_key=(best[1], best[2]) if best else None)
@@ -524,6 +569,8 @@ def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int,
         result._ranker = search.make_window_ranker(searcher, merged.records, result.summary)
     result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
                       'decode_columns_s': time.perf_counter() - t2}
+    if headroom:
+        result.timings['headroom_s'] = merged.headroom_s
     return result
 
 

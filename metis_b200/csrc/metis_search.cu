@@ -23,7 +23,7 @@
 //   homo_cost_kernel      a17: one thread per UniformPlan
 //   homo_breakdown_kernel the same with the cost terms and per-stage memory
 //   layer_balance_kernel  a10 alone, for unit parity
-//   (rank_records_kernel, the stable record sort, lives in metis_rank.cu)
+//   (rank_records_kernel, the stable record sort, lives in metis_rank.cu; the headroom select / front in metis_select.cu)
 //
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (no FMA contraction: parity).
 #include <cuda_runtime.h>
@@ -32,6 +32,8 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include "metis_eval.cuh"
 #include "metis_coop.cuh"
@@ -292,6 +294,7 @@ struct DeviceSink {
     __device__ DeviceSink(const DeviceOut &out)
         : o(out), n_part(0), n_run(0), n_key(0), best_cost(INFINITY), best_ord(0xFFFFFFFFu), best_step(0xFFFFu),
           best_meta(0), leader(true) {}
+    __device__ DeviceSink(const DeviceOut &out, double *) : DeviceSink(out) {}   // the kernels without headroom
 #ifdef METIS_PROFILE_PHASES
     __device__ void phase(int id) { bulk_mark(0xFFFFFFFFu, id); }   // bulk round: called by all 32 lanes
 #else
@@ -309,6 +312,12 @@ struct DeviceSink {
         atomicMin(&o.counters[4], key);
     }
     __device__ void emit(const PlanDesc &pd, int step, int nrep, double cost, const uint8_t *tpc, const uint16_t *part) {
+        emit_with(pd, step, nrep, cost, tpc, part, [](unsigned long long) {});
+    }
+    // `also(slot)`: more per-record output, written after the record itself
+    template <class Also>
+    __device__ void emit_with(const PlanDesc &pd, int step, int nrep, double cost, const uint8_t *tpc,
+                              const uint16_t *part, const Also &also) {
         if (!leader) return;
         const unsigned long long slot = atomicAdd(&o.counters[0], 1ULL);
         if ((long long)slot < o.capacity) {
@@ -316,6 +325,7 @@ struct DeviceSink {
             r.cost = cost; r.ordinal = pd.ordinal; r.step = (uint16_t)step;
             r.num_repartition = (uint8_t)nrep; r.num_stage = (uint8_t)pd.S;
             o.records[slot] = r;
+            also(slot);
             if (o.detail) {
                 uint8_t *d = o.detail + (size_t)slot * o.detail_stride;
                 for (int s = 0; s < pd.S; ++s) { d[s] = (uint8_t)(pd.row[s] - tpc[s]); d[pd.S + s] = tpc[s]; }
@@ -328,6 +338,26 @@ struct DeviceSink {
         }
     }
 };
+
+// Sink of the search kernels compiled with headroom (template flag HEAD): DeviceSink, and each record's memory headroom
+// next to it.  Headroom is a compile-time choice so that the kernels without it are exactly DeviceSink's.
+struct HeadroomSink : DeviceSink {
+    double *headroom;               // aligned with the records
+    // the evaluator's Scratch::mstate: at an emit it holds the memory_state of the attempt just accepted (memory_phase
+    // and memory_phase_coop return 1 only with it set; nothing writes it between that and the emit)
+    const double *state;
+    __device__ HeadroomSink(const DeviceOut &out, double *h) : DeviceSink(out), headroom(h), state(nullptr) {}
+    __device__ void emit(const PlanDesc &pd, int step, int nrep, double cost, const uint8_t *tpc, const uint16_t *part) {
+        emit_with(pd, step, nrep, cost, tpc, part, [&](unsigned long long slot) {
+            double m = state[0];                             // every stage, costed or not; lowest first, like
+            for (int s = 1; s < pd.S; ++s)                   // BreakdownEvaluator's min_headroom
+                if (state[s] < m) m = state[s];
+            headroom[slot] = m;
+        });
+    }
+};
+template <bool HEAD>
+using SearchSink = typename std::conditional<HEAD, HeadroomSink, DeviceSink>::type;
 
 // End of a search kernel: counters (warp reduce, one atomic per warp) and the block's best candidate:
 // argmin (cost, ordinal, step) by __shfl_xor_sync inside the warp, then across the warps through shared memory.
@@ -481,19 +511,20 @@ het_scatter_kernel(const SearchLists ls) {
     }
 }
 
-template <int MAXS, int MAXL, bool ONE>
+template <int MAXS, int MAXL, bool ONE, bool HEAD>
 __global__ void __launch_bounds__(kThreads, (MAXS <= 64 ? METIS_MIN_BLOCKS : ONE ? METIS_MIN_BLOCKS_BIG_ONE : METIS_MIN_BLOCKS_BIG))
 het_first_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ MetisPlanSpace sp,
                  const __grid_constant__ BlobLayout lay, const uint8_t *__restrict__ blob, const int use_smem,
-                 const __grid_constant__ DeviceOut out, const SearchLists ls, const int best_slot) {
+                 const __grid_constant__ DeviceOut out, const SearchLists ls, const int best_slot, double *headroom) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
     __shared__ Tables s_tables;
-    DeviceSink sink(out);
+    SearchSink<HEAD> sink(out, headroom);
     const unsigned int n = ls.ctl[0];
     if ((long long)n >= ls.bulk_min) {
         const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
         Scratch<MAXS, MAXL> w;
+        if constexpr (HEAD) sink.state = w.mstate;
         const int lane = threadIdx.x & 31;
         for (;;) {                                           // batches of 32 plans, longest stage counts first
             unsigned int fetched = 0;
@@ -559,22 +590,24 @@ struct alignas(16) ChainScratch {
     CoopMail mail;
 };
 
+
 // 64 registers per thread: 32 resident warps per SM in blocks of 16 warps (tables staged once per block)
-template <int MAXS, int MAXL, bool ONE>
+template <int MAXS, int MAXL, bool ONE, bool HEAD>
 __global__ void __launch_bounds__(512, 2)
 het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ MetisPlanSpace sp,
                  const __grid_constant__ BlobLayout lay, const uint8_t *__restrict__ blob, const int use_smem,
                  const unsigned int scratch_off, const __grid_constant__ DeviceOut out, const SearchLists ls,
-                 const int best_slot) {
+                 const int best_slot, double *headroom) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
     __shared__ Tables s_tables;
     WarpCoop::prof_init();                                   // (phase clock build only; published by block_tables)
     const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
-    DeviceSink sink(out);
+    SearchSink<HEAD> sink(out, headroom);
     const int lane = threadIdx.x & 31;
     sink.leader = lane == 0;
     ChainScratch<MAXS, MAXL> *cs = reinterpret_cast<ChainScratch<MAXS, MAXL> *>(smem + scratch_off) + (threadIdx.x >> 5);
+    if constexpr (HEAD) sink.state = cs->w.mstate;           // read by the leader after run_chain's x.sync()
     const unsigned int n_adm = ls.ctl[0];
     const bool bulk = (long long)n_adm >= ls.bulk_min;
     const uint4 *list = ls.b;                                // sorted: by chain hint after a bulk round, else by stage count
@@ -916,10 +949,10 @@ static Workspace carve(void *ws, const BlobLayout &lay) {
 }  // extern "C"
 
 // Launch configuration of one search: which instantiation, how the tables are staged, block shapes.
-template <int MAXS, int MAXL, bool ONE>
+template <int MAXS, int MAXL, bool ONE, bool HEAD>
 static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg, const MetisShard &sh,
-                         const BlobLayout &lay, const Workspace &ws, const DeviceOut &out, int64_t slots,
-                         cudaStream_t stream) {
+                         const BlobLayout &lay, const Workspace &ws, const DeviceOut &out, double *headroom,
+                         int64_t slots, cudaStream_t stream) {
     cudaError_t e;
     int dev = 0, sms = 0, smem_optin = 0;
     cudaGetDevice(&dev);
@@ -939,7 +972,7 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     ls.save_cap = (unsigned int)save_slots(cap);
 
     // ---- chain kernel: warps per block chosen so that tables + per-warp scratch fill the SM with warps ----
-    auto chain = het_chain_kernel<MAXS, MAXL, ONE>;
+    auto chain = het_chain_kernel<MAXS, MAXL, ONE, HEAD>;
     const size_t per_warp = sizeof(ChainScratch<MAXS, MAXL>);
     int chain_smem_tables = (int)lay.total <= blob_max;
     int chain_threads = 0, chain_per_sm = 0;
@@ -970,7 +1003,7 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     int64_t chain_grid = (int64_t)sms * chain_per_sm;
 
     // ---- bulk round ----
-    auto first = het_first_kernel<MAXS, MAXL, ONE>;
+    auto first = het_first_kernel<MAXS, MAXL, ONE, HEAD>;
     int first_smem_tables = (int)lay.total <= blob_max && blob_pad <= (unsigned int)smem_optin;
     size_t first_dyn = first_smem_tables ? blob_pad : 0;
     e = cudaFuncSetAttribute(first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_dyn);
@@ -993,10 +1026,11 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
         int64_t scatter_blocks = (slots + 255) / 256;
         if (scatter_blocks > 8LL * sms) scatter_blocks = 8LL * sms;
         het_scatter_kernel<<<(unsigned)scatter_blocks, 256, 0, stream>>>(ls);
-        first<<<(unsigned)first_grid, kThreads, first_dyn, stream>>>(p_arg, s_arg, lay, ws.blob, first_smem_tables, out, ls, 0);
+        first<<<(unsigned)first_grid, kThreads, first_dyn, stream>>>(p_arg, s_arg, lay, ws.blob, first_smem_tables, out, ls, 0,
+                                                                  headroom);
         het_order_kernel<<<(unsigned)(2 * sms), 256, 0, stream>>>(ls);
         chain<<<(unsigned)chain_grid, chain_threads, chain_dyn, stream>>>(p_arg, s_arg, lay, ws.blob, chain_smem_tables,
-                                                                         chain_off, out, ls, (int)first_grid);
+                                                                         chain_off, out, ls, (int)first_grid, headroom);
         e = cudaGetLastError();
         if (e != cudaSuccess) return cuda_fail(e, "search kernels");
     }
@@ -1011,11 +1045,36 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     return METIS_OK;
 }
 
+// three instantiations: per-warp scratch of the chain kernel (and per-thread scratch of the bulk round)
+// sized for S <= 64 / L <= 128, S <= 96 / L <= 128, and the compiled limits
+// ... each once for single-type clusters (no mixed-type code at all) and once for the general case
+template <bool HEAD>
+static int launch_tier(const MetisProblem &p, const MetisPlanSpace &sp, const MetisShard &sh, const BlobLayout &lay,
+                       const Workspace &ws, const DeviceOut &out, double *headroom, int64_t slots, cudaStream_t stream) {
+    const bool one = p.num_types == 1;
+    if (sp.max_stage <= 64 && p.num_layers <= 128)
+        return one ? launch_search<64, 128, true, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream)
+                   : launch_search<64, 128, false, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream);
+    if (sp.max_stage <= 96 && p.num_layers <= 128)
+        return one ? launch_search<96, 128, true, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream)
+                   : launch_search<96, 128, false, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream);
+    return one ? launch_search<kMaxS, kMaxL, true, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream)
+               : launch_search<kMaxS, kMaxL, false, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream);
+}
+
 extern "C" {
 
 int metis_het_search(const MetisProblem *problem, const MetisPlanSpace *space, const MetisShard *shard,
                      MetisRecord *records, int64_t capacity, uint8_t *detail, int32_t detail_stride,
                      void *workspace, int64_t workspace_bytes, MetisSearchSummary *summary, void *stream_) {
+    return metis_het_search_headroom(problem, space, shard, records, capacity, detail, detail_stride, nullptr, workspace,
+                                     workspace_bytes, summary, stream_);
+}
+
+int metis_het_search_headroom(const MetisProblem *problem, const MetisPlanSpace *space, const MetisShard *shard,
+                              MetisRecord *records, int64_t capacity, uint8_t *detail, int32_t detail_stride,
+                              double *headroom, void *workspace, int64_t workspace_bytes, MetisSearchSummary *summary,
+                              void *stream_) {
     int rc = check_problem(problem);
     if (rc) return rc;
     if (!space || !shard || !workspace || !summary) return arg_fail("NULL argument");
@@ -1030,6 +1089,7 @@ int metis_het_search(const MetisProblem *problem, const MetisPlanSpace *space, c
     if (space->rows_bytes < 0 || space->rows_bytes > 0xFFFFFFFFLL) return arg_fail("row tables must be smaller than 4 GiB (geometry word)");
     if (detail && detail_stride < 3 * space->max_stage + 1) return arg_fail("detail_stride too small (3 * max_stage + 1)");
     if (capacity < 0 || (capacity > 0 && !records)) return arg_fail("records/capacity mismatch");
+    if (headroom && !records) return arg_fail("headroom without records");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const BlobLayout lay = make_layout(*problem);
     const int64_t slots = shard_plan_slots(space->num_plans, shard);
@@ -1053,19 +1113,8 @@ int metis_het_search(const MetisProblem *problem, const MetisPlanSpace *space, c
     DeviceOut out;
     out.records = records; out.capacity = capacity; out.detail = detail; out.detail_stride = detail_stride;
     out.counters = ws.counters; out.block_best = ws.block_best;
-    // three instantiations: per-warp scratch of the chain kernel (and per-thread scratch of the bulk round)
-    // sized for S <= 64 / L <= 128, S <= 96 / L <= 128, and the compiled limits
-    // ... each once for single-type clusters (no mixed-type code at all) and once for the general case
-    const bool one = problem->num_types == 1;
-    if (space->max_stage <= 64 && problem->num_layers <= 128)
-        rc = one ? launch_search<64, 128, true>(*problem, *space, *shard, lay, ws, out, slots, stream)
-                 : launch_search<64, 128, false>(*problem, *space, *shard, lay, ws, out, slots, stream);
-    else if (space->max_stage <= 96 && problem->num_layers <= 128)
-        rc = one ? launch_search<96, 128, true>(*problem, *space, *shard, lay, ws, out, slots, stream)
-                 : launch_search<96, 128, false>(*problem, *space, *shard, lay, ws, out, slots, stream);
-    else
-        rc = one ? launch_search<kMaxS, kMaxL, true>(*problem, *space, *shard, lay, ws, out, slots, stream)
-                 : launch_search<kMaxS, kMaxL, false>(*problem, *space, *shard, lay, ws, out, slots, stream);
+    rc = headroom ? launch_tier<true>(*problem, *space, *shard, lay, ws, out, headroom, slots, stream)
+                  : launch_tier<false>(*problem, *space, *shard, lay, ws, out, nullptr, slots, stream);
     if (rc) return rc;
     e = cudaMemcpyAsync(summary, ws.summary, sizeof(MetisSearchSummary), cudaMemcpyDeviceToHost, stream);
     if (e != cudaSuccess) return cuda_fail(e, "copy summary");

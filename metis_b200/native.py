@@ -92,7 +92,8 @@ SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 
            'metis_homo_breakdown', 'metis_layer_balance', 'metis_enum_device_groups',
            'metis_enum_device_group_tables', 'metis_sort_workspace_bytes', 'metis_sort_records',
            'metis_enum_compositions', 'metis_generate_rows', 'metis_list_workspace_bytes', 'metis_list_stages',
-           'metis_list_window']
+           'metis_list_window', 'metis_het_search_headroom', 'metis_headroom_workspace_bytes', 'metis_headroom_select',
+           'metis_headroom_front']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -122,6 +123,18 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_het_search.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisShard),
                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64,
                                      C.c_void_p, C.c_void_p]
+    lib.metis_het_search_headroom.restype = C.c_int
+    lib.metis_het_search_headroom.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisShard),
+                                              C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                              C.c_int64, C.c_void_p, C.c_void_p]
+    lib.metis_headroom_workspace_bytes.restype = C.c_int64
+    lib.metis_headroom_workspace_bytes.argtypes = [C.c_int64]
+    lib.metis_headroom_select.restype = C.c_int
+    lib.metis_headroom_select.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_int64, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.metis_headroom_front.restype = C.c_int
+    lib.metis_headroom_front.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_int64, C.c_void_p]
     lib.metis_het_detail.restype = C.c_int
     lib.metis_het_detail.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.c_void_p, C.c_int64,
                                      C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]

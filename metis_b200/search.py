@@ -8,6 +8,8 @@ include/metis_b200.h.  There is no CPU path: without CUDA these functions raise.
 from __future__ import annotations
 
 import ctypes as C
+import math
+import time
 import weakref
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -166,6 +168,9 @@ class HetSearchOutput:
     rank_order: Optional[np.ndarray] = None               # uint32: records[rank_order] = sorted(..., key=cost), stable
     detail_dev: Optional[torch.Tensor] = None             # uint8 [n, stride] on the device
     records_dev: Optional[torch.Tensor] = None            # int64 [2n]: the sorted records on the device
+    headroom: Optional[np.ndarray] = None                 # float64 [n] aligned with records (want_headroom)
+    headroom_dev: Optional[torch.Tensor] = None           # the same on the device
+    headroom_s: float = 0.0                               # host time spent ordering and copying the headroom
 
 
 class HetSearcher:
@@ -173,8 +178,12 @@ class HetSearcher:
 
     def __init__(self, dp: DeviceProblem, rank: int = 0, world: int = 1, tile: int = 128,
                  want_records: bool = True, want_detail: bool = False, capacity: Optional[int] = None,
-                 want_ranking: bool = False, detail_to_host: bool = True, detail_stride: Optional[int] = None):
+                 want_ranking: bool = False, detail_to_host: bool = True, detail_stride: Optional[int] = None,
+                 want_headroom: bool = False):
+        """``want_headroom``: the search also writes each record's memory headroom (metis_het_search_headroom)."""
         self.dp = dp
+        self.want_headroom = want_headroom and want_records
+        self.headroom = None
         self.want_ranking = want_ranking and want_records
         self._sort_ws = None
         self.shard = native.MetisShard(rank, world, tile, 0)
@@ -218,6 +227,7 @@ class HetSearcher:
         self.capacity = capacity
         with torch.cuda.device(dev):
             self.records = torch.empty(capacity * 2, dtype=torch.int64, device=dev)
+            self.headroom = torch.empty(capacity, dtype=torch.float64, device=dev) if self.want_headroom else None
             self.detail = (torch.empty((capacity, self.detail_stride), dtype=torch.uint8, device=dev)
                            if self.want_detail else None)
 
@@ -225,13 +235,20 @@ class HetSearcher:
         """Enqueue pack + search + finalize + summary copy on ``stream`` (asynchronous)."""
         dp = self.dp
         s = stream or torch.cuda.current_stream(dp.device)
-        rc = dp.lib.metis_het_search(
-            C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard),
-            C.c_void_p(self.records.data_ptr() if self.records is not None else 0), C.c_int64(self.capacity),
-            C.c_void_p(self.detail.data_ptr() if self.detail is not None else 0), C.c_int32(self.detail_stride),
-            C.c_void_p(self.workspace.data_ptr()), C.c_int64(self.workspace.numel()),
-            C.c_void_p(self.summary_host.data_ptr()), C.c_void_p(s.cuda_stream))
-        native.check(rc, 'metis_het_search')
+        if self.want_headroom and self.records is not None and self.headroom is None:
+            with torch.cuda.device(dp.device):
+                self.headroom = torch.empty(self.capacity, dtype=torch.float64, device=dp.device)
+        common = (C.c_void_p(self.records.data_ptr() if self.records is not None else 0), C.c_int64(self.capacity),
+                  C.c_void_p(self.detail.data_ptr() if self.detail is not None else 0), C.c_int32(self.detail_stride))
+        tail = (C.c_void_p(self.workspace.data_ptr()), C.c_int64(self.workspace.numel()),
+                C.c_void_p(self.summary_host.data_ptr()), C.c_void_p(s.cuda_stream))
+        if self.want_headroom:
+            rc = dp.lib.metis_het_search_headroom(C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard),
+                                                  *common, C.c_void_p(self.headroom.data_ptr()), *tail)
+            native.check(rc, 'metis_het_search_headroom')
+        else:
+            rc = dp.lib.metis_het_search(C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard), *common, *tail)
+            native.check(rc, 'metis_het_search')
 
     def summary(self) -> native.MetisSearchSummary:
         return native.MetisSearchSummary.from_buffer_copy(self.summary_host.numpy().tobytes())
@@ -287,12 +304,13 @@ class HetSearcher:
             if sm.num_records > 0:
                 b = sm.best
                 best = (float(b.cost), int(b.ordinal), int(b.step), int(b.num_repartition), int(b.num_stage))
-            records = detail = rank_order = detail_dev = records_dev = None
+            records = detail = rank_order = detail_dev = records_dev = headroom = headroom_dev = None
+            headroom_s = 0.0
             d2h = C.sizeof(native.MetisSearchSummary)
             if self.want_records:
                 n = int(sm.num_records)
                 # estimate_costs order = (ordinal, step): rank_records_kernel, in place
-                order = self.sort_records(n, native.SORT_POSITION, s, want_perm=self.want_detail)
+                order = self.sort_records(n, native.SORT_POSITION, s, want_perm=self.want_detail or self.want_headroom)
                 records_dev = self.records[:2 * n]
                 records = self._to_host('records', records_dev, s).view(native.RECORD_DTYPE)
                 d2h += n * 16
@@ -301,13 +319,20 @@ class HetSearcher:
                     if self.detail_to_host:
                         detail = self._to_host('detail', detail_dev, s).reshape(n, self.detail_stride)
                         d2h += n * self.detail_stride
+                if self.want_headroom:                       # the same permutation as the detail rows
+                    t = time.perf_counter()
+                    headroom_dev = self.headroom[:n].index_select(0, order.long())
+                    headroom = self._to_host('headroom', headroom_dev, s).view(np.float64)
+                    d2h += n * 8
+                    headroom_s = time.perf_counter() - t
                 if self.want_ranking:
                     # sorted(estimate_costs, key=cost): stable by cost on a copy of the ordered records
                     by_cost = self.records[:2 * n].clone()
                     perm = self.sort_records(n, native.SORT_BY_COST_STABLE, s, want_perm=True, buf=by_cost)
                     rank_order = self._to_host('rank', perm, s).view(np.uint32)
                     d2h += n * 4
-        return HetSearchOutput(out_summary, best, records, detail, d2h, rank_order, detail_dev, records_dev)
+        return HetSearchOutput(out_summary, best, records, detail, d2h, rank_order, detail_dev, records_dev, headroom,
+                               headroom_dev, headroom_s)
 
     def sort_records(self, n: int, mode: int, stream: torch.cuda.Stream, want_perm: bool = False, buf=None):
         """metis_sort_records on the first n records (device, in place, asynchronous on ``stream``); returns the
@@ -371,8 +396,11 @@ class Candidates:
 
     def __init__(self, records: np.ndarray, detail: Optional[np.ndarray], space: flatten.FlatPlanSpace,
                  node_sequences: Sequence[Tuple], detail_dev: Optional[torch.Tensor] = None,
-                 rows_dev: Optional[torch.Tensor] = None, problem: Optional[flatten.FlatProblem] = None):
+                 rows_dev: Optional[torch.Tensor] = None, problem: Optional[flatten.FlatProblem] = None,
+                 headroom: Optional[np.ndarray] = None):
         self.records = records
+        self.headroom = headroom              # float64 per record (a search with headroom), else None
+        self.device = rows_dev.device if rows_dev is not None else None   # where the search ran (None: not known)
         self.space = space
         self.problem = problem                # the tables breakdown() replays the candidates on
         self.node_sequences = [tuple(s) for s in node_sequences]
@@ -590,6 +618,8 @@ class WindowedOutput:
     records: np.ndarray
     bases: np.ndarray                                     # int64 per window searched
     firsts: np.ndarray                                    # int64, one more than windows searched
+    headroom: Optional[np.ndarray] = None                 # float64 aligned with records, when the windows had it
+    headroom_s: float = 0.0
 
 
 class WindowMerge:
@@ -597,16 +627,22 @@ class WindowMerge:
     step), the fatal ordinal made global.  ``add`` returns True at the first window that reports a fatal plan: the
     reference dies at that plan (quirk Q8), so later windows are not searched."""
 
-    def __init__(self, num_windows: int):
+    def __init__(self, num_windows: int, with_headroom: bool = False):
+        """``with_headroom``: the windows carry headroom, so an empty result gets an empty headroom array."""
+        self.with_headroom = with_headroom
         self.summary: Dict[str, object] = {k: 0 for k in _SUMMED_KEYS}
         self.summary.update(fatal_ordinal=_NO_FATAL, fatal_code=0, fatal_aux=0, num_windows=num_windows,
                             windows_searched=0, instantiation=[])
         self.best = None
         self._records: List[np.ndarray] = []
+        self._headroom: List[np.ndarray] = []
+        self.headroom_s = 0.0
         self.bases: List[int] = []
         self.firsts: List[int] = [0]
 
-    def add(self, base: int, summary: Dict[str, int], best, records: Optional[np.ndarray]) -> bool:
+    def add(self, base: int, summary: Dict[str, int], best, records: Optional[np.ndarray],
+            headroom: Optional[np.ndarray] = None) -> bool:
+        """``headroom``: the window's per-record headroom, aligned with ``records`` (give it for every window or none)."""
         for k in _SUMMED_KEYS:
             self.summary[k] += int(summary.get(k, 0))
         self.summary['windows_searched'] += 1
@@ -619,6 +655,8 @@ class WindowMerge:
         n = 0 if records is None else len(records)
         if n:
             self._records.append(records)
+            if headroom is not None:
+                self._headroom.append(headroom)
         self.bases.append(int(base))
         self.firsts.append(self.firsts[-1] + n)
         if int(summary.get('fatal_ordinal', _NO_FATAL)) != _NO_FATAL:
@@ -629,8 +667,12 @@ class WindowMerge:
 
     def result(self) -> WindowedOutput:
         rec = np.concatenate(self._records) if self._records else np.zeros(0, dtype=native.RECORD_DTYPE)
+        head = None
+        if self._headroom or (self.with_headroom and not self._records):
+            head = np.concatenate(self._headroom) if self._headroom else np.zeros(0)
+            assert len(head) == len(rec), 'headroom given for some windows only'
         return WindowedOutput(dict(self.summary), self.best, rec, np.asarray(self.bases, dtype=np.int64),
-                              np.asarray(self.firsts, dtype=np.int64))
+                              np.asarray(self.firsts, dtype=np.int64), head, self.headroom_s)
 
 
 def window_cost_model(problem: flatten.FlatProblem, lib=None) -> Tuple[float, float, float, float]:
@@ -668,24 +710,27 @@ def agree_budget(budget: float, device) -> float:
 
 
 def search_windows(problem: flatten.FlatProblem, windows: Sequence[flatten.PlanWindow], device=None, rank: int = 0,
-                   world: int = 1, tile: int = 128) -> Tuple[WindowedOutput, DeviceProblem, 'HetSearcher']:
+                   world: int = 1, tile: int = 128, headroom: bool = False
+                   ) -> Tuple[WindowedOutput, DeviceProblem, 'HetSearcher']:
     """Search the windows in ordinal order in ONE DeviceProblem arena (sized for every window up front) with ONE
     HetSearcher (the shard's tiles of every window, workspace sized for the window with the most plans), records only,
     and merge on the host (WindowMerge).  Afterwards the searcher keeps only what rebuilding candidates needs
     (metis_het_detail's workspace): the work lists and the record buffer are released."""
     dp = DeviceProblem(problem, windows[0].space, device, reserve=windows)
-    searcher = HetSearcher(dp, rank, world, tile, want_records=True, want_detail=False)
+    searcher = HetSearcher(dp, rank, world, tile, want_records=True, want_detail=False, want_headroom=headroom)
     searcher.reserve_workspace(max(w.space.num_plans for w in windows))
-    merge = WindowMerge(len(windows))
+    merge = WindowMerge(len(windows), with_headroom=headroom)
     for w in windows:
         if dp.space is not w.space:                           # the first window was uploaded by the constructor
             dp.reload(problem, w.space)
             dp.upload()
             searcher.rebind()
         out = searcher.run()
-        if merge.add(w.base, out.summary, out.best, np.array(out.records) if out.records is not None else None):
+        merge.headroom_s += out.headroom_s
+        if merge.add(w.base, out.summary, out.best, np.array(out.records) if out.records is not None else None,
+                     np.array(out.headroom) if out.headroom is not None else None):
             break
-    searcher.records = searcher.workspace = None
+    searcher.records = searcher.workspace = searcher.headroom = None
     searcher.capacity = 0
     with torch.cuda.device(dp.device):
         searcher.workspace = torch.empty(dp.workspace_bytes(0), dtype=torch.uint8, device=dp.device)
@@ -723,8 +768,26 @@ def gather_window_records(merged: WindowedOutput, device) -> WindowedOutput:
     got = torch.empty(world * cap * 2, dtype=torch.int64, device=device)
     dist.all_gather_into_tensor(got, mine)
     flat = got.cpu().numpy().view(native.RECORD_DTYPE).reshape(world, cap)
-    rec, firsts = merge_rank_windows(all_counts, [flat[r] for r in range(world)])
-    return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts)
+    if merged.headroom is None:
+        rec, firsts = merge_rank_windows(all_counts, [flat[r] for r in range(world)])
+        return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts)
+    # the headroom travels padded like the records, and is merged with them as one more field of each record
+    mine_h = torch.zeros(cap, dtype=torch.float64, device=device)
+    if n_local:
+        mine_h[:n_local] = torch.from_numpy(np.ascontiguousarray(merged.headroom)).to(device)
+    got_h = torch.empty(world * cap, dtype=torch.float64, device=device)
+    dist.all_gather_into_tensor(got_h, mine_h)
+    flat_h = got_h.cpu().numpy().reshape(world, cap)
+    both = np.zeros((world, cap), dtype=native.RECORD_DTYPE + [('headroom', '<f8')])
+    for f, _ in native.RECORD_DTYPE:
+        both[f] = flat[f]
+    both['headroom'] = flat_h
+    merged_both, firsts = merge_rank_windows(all_counts, [both[r] for r in range(world)])
+    rec = np.zeros(len(merged_both), dtype=native.RECORD_DTYPE)
+    for f, _ in native.RECORD_DTYPE:
+        rec[f] = merged_both[f]
+    return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts,
+                          np.ascontiguousarray(merged_both['headroom']), merged.headroom_s)
 
 
 def make_window_ranker(searcher: 'HetSearcher', records: np.ndarray, summary: Dict):
@@ -761,8 +824,10 @@ class WindowedCandidates:
 
     def __init__(self, records: np.ndarray, bases: np.ndarray, firsts: np.ndarray,
                  windows: Sequence[flatten.PlanWindow], problem: flatten.FlatProblem, node_sequences: Sequence[Tuple],
-                 searcher: 'HetSearcher'):
+                 searcher: 'HetSearcher', headroom: Optional[np.ndarray] = None):
         self.records = records
+        self.headroom = headroom              # float64 per record (a search with headroom), else None
+        self.device = searcher.dp.device      # where the search ran
         self.cost = records['cost']
         self.bases = bases
         self.firsts = firsts
@@ -922,6 +987,76 @@ def make_ranker(searcher: 'HetSearcher', records_dev: torch.Tensor):
     return rank
 
 
+def check_threshold(min_headroom) -> float:
+    """A headroom threshold must be a finite real number (MB)."""
+    try:
+        x = float(min_headroom)
+    except (TypeError, ValueError):
+        raise ValueError(f'min_headroom must be a finite number, not {min_headroom!r}') from None
+    if isinstance(min_headroom, (bool, np.bool_)) or not math.isfinite(x):
+        raise ValueError(f'min_headroom must be a finite number, not {min_headroom!r}')
+    return x
+
+
+class HeadroomIndex:
+    """The records, their headroom and the ranked order of one result on the device, for metis_headroom_select and
+    metis_headroom_front (uploaded once, on the first query)."""
+
+    def __init__(self, records: np.ndarray, headroom: np.ndarray, rank_order: np.ndarray, device=None):
+        self.device = _require_cuda(device)
+        self.lib = native.load_library()
+        self.n = len(records)
+        if not (len(headroom) == len(rank_order) == self.n):
+            raise ValueError('records, headroom and rank order differ in length')
+        with torch.cuda.device(self.device):
+            up = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).to(self.device)
+            self.records = up(records)
+            self.headroom = up(np.asarray(headroom, dtype=np.float64))
+            self.rank = up(np.asarray(rank_order, dtype=np.uint32))
+            need = int(self.lib.metis_headroom_workspace_bytes(C.c_int64(self.n)))
+            self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
+            self.out = torch.empty(max(self.n, 1), dtype=torch.int32, device=self.device)
+        self.count = torch.zeros(1, dtype=torch.int64).pin_memory()
+
+    def launch_select(self, min_headroom: float, k: int, stream) -> None:
+        rc = self.lib.metis_headroom_select(C.c_void_p(self.headroom.data_ptr()), C.c_void_p(self.rank.data_ptr()),
+                                            C.c_int64(self.n), C.c_double(min_headroom), C.c_int64(k),
+                                            C.c_void_p(self.out.data_ptr()), C.c_void_p(self.count.data_ptr()),
+                                            C.c_void_p(self.workspace.data_ptr()), C.c_int64(self.workspace.numel()),
+                                            C.c_void_p(stream.cuda_stream))
+        native.check(rc, 'metis_headroom_select')
+
+    def launch_front(self, stream) -> None:
+        rc = self.lib.metis_headroom_front(C.c_void_p(self.records.data_ptr()), C.c_void_p(self.headroom.data_ptr()),
+                                           C.c_void_p(self.rank.data_ptr()), C.c_int64(self.n),
+                                           C.c_void_p(self.out.data_ptr()), C.c_void_p(self.count.data_ptr()),
+                                           C.c_void_p(self.workspace.data_ptr()), C.c_int64(self.workspace.numel()),
+                                           C.c_void_p(stream.cuda_stream))
+        native.check(rc, 'metis_headroom_front')
+
+    def select(self, min_headroom: float, k: Optional[int] = None) -> Tuple[np.ndarray, int]:
+        """(positions of the first ``k`` (default: all) ranked entries with headroom >= min_headroom, how many
+        qualify in all)."""
+        x = check_threshold(min_headroom)
+        if k is not None and int(k) < 0:
+            raise ValueError(f'k must be >= 0 with min_headroom, not {k}')
+        k = self.n if k is None else min(int(k), self.n)
+        with torch.cuda.device(self.device):
+            s = torch.cuda.current_stream(self.device)
+            self.launch_select(x, k, s)
+            s.synchronize()
+            total = int(self.count[0])
+            return self.out[:min(k, total)].cpu().numpy().view(np.uint32).astype(np.int64), total
+
+    def front(self) -> np.ndarray:
+        """Positions of the cost / headroom Pareto front, by ascending cost."""
+        with torch.cuda.device(self.device):
+            s = torch.cuda.current_stream(self.device)
+            self.launch_front(s)
+            s.synchronize()
+            return self.out[:int(self.count[0])].cpu().numpy().view(np.uint32).astype(np.int64)
+
+
 def gather_records(out: HetSearchOutput, searcher: HetSearcher, want_rank: bool = True,
                    counts: Optional[List[int]] = None) -> HetSearchOutput:
     """Every rank receives every rank's records (+ detail rows): padded tensor all_gathers over NCCL (no pickling),
@@ -950,6 +1085,13 @@ def gather_records(out: HetSearchOutput, searcher: HetSearcher, want_rank: bool 
             det_g = torch.empty((world * cap, stride), dtype=torch.uint8, device=dev)
             dist.all_gather_into_tensor(det_g, det_pad)
             det_all = torch.cat([det_g[cap * r:cap * r + counts[r]] for r in range(world)])
+        head_all = None
+        if out.headroom_dev is not None:                      # padded like the records
+            head_pad = torch.zeros(cap, dtype=torch.float64, device=dev)
+            head_pad[:n_local] = out.headroom_dev
+            head_g = torch.empty(world * cap, dtype=torch.float64, device=dev)
+            dist.all_gather_into_tensor(head_g, head_pad)
+            head_all = torch.cat([head_g[cap * r:cap * r + counts[r]] for r in range(world)])
         n = sum(counts)
         s = torch.cuda.current_stream(dev)
         perm = searcher.sort_records(n, native.SORT_POSITION, s, want_perm=True, buf=rec_all)
@@ -963,8 +1105,12 @@ def gather_records(out: HetSearchOutput, searcher: HetSearcher, want_rank: bool 
         detail = None
         if detail_dev is not None and searcher.detail_to_host:
             detail = searcher._to_host('detail_all', detail_dev, s).reshape(n, stride)
+        headroom = headroom_dev = None
+        if head_all is not None:
+            headroom_dev = head_all.index_select(0, perm.long())
+            headroom = searcher._to_host('headroom_all', headroom_dev, s).view(np.float64)
     return HetSearchOutput(out.summary, out.best, records, detail, out.d2h_bytes, rank_order, detail_dev,
-                           rec_all[:2 * n])
+                           rec_all[:2 * n], headroom, headroom_dev, out.headroom_s)
 
 
 # ---------------------------------------------------------------------------------------------
