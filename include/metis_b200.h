@@ -158,8 +158,27 @@ typedef struct MetisSearchSummary {
     uint64_t reserved[6];         /* [0] plans admitted (have a valid first strategy), [1] plans handed from the
                                      bulk round to the chain kernel, [2] the instantiation of the search
                                      kernels that ran: MAXS | MAXL << 16 | ONE << 32 (scratch sized for
-                                     MAXS stages / MAXL layers; ONE = single-type cluster); rest 0      */
+                                     MAXS stages / MAXL layers; ONE = single-type cluster), [3] the
+                                     out-of-memory partition attempts of a search with misses
+                                     (metis_het_search_outputs; exact past the capacity, 0 without); rest 0 */
 } MetisSearchSummary;
+
+/*
+ * 16-byte record per out-of-memory partition attempt (metis_het_search_outputs): one pass of the partition_layer loop
+ * whose memory test fails (model/load_balancer.py:57-63,127-143), the third attempt and the attempts whose re-weighting
+ * is None included.  deficit, ordinal and key sit where MetisRecord keeps cost, ordinal and step, so
+ * metis_sort_records orders misses too: METIS_SORT_POSITION by (ordinal, call, attempt), the order the reference
+ * prints them; METIS_SORT_RANKED closest first (smallest deficit), ties in that order.
+ */
+typedef struct MetisMiss {
+    double deficit;               /* -min_s memory_state[s] (MB), > 0                                  */
+    uint32_t ordinal;             /* inter-stage plan ordinal                                       */
+    uint16_t key;                 /* call << 2 | attempt: call = 0-based partition_layer call of the plan, attempt 1..3;
+                                     a plan makes at most num_stage * floor(log2(max_tp)) + 1 <= 3 841 calls (every
+                                     strategy of its chain doubles one stage's tp), so the call fits in 14 bits */
+    uint8_t stage;                /* lowest stage attaining that minimum                            */
+    uint8_t num_stage;
+} MetisMiss;
 
 /* Shard of the ordinal space evaluated by one call (multi-GPU: rank r of n, interleaved tiles). */
 typedef struct MetisShard {
@@ -214,6 +233,17 @@ int metis_het_search_headroom(const MetisProblem *problem, const MetisPlanSpace 
                               MetisRecord *records, int64_t capacity, uint8_t *detail, int32_t detail_stride,
                               double *headroom, void *workspace, int64_t workspace_bytes, MetisSearchSummary *summary,
                               void *stream);
+
+/*
+ * metis_het_search_headroom that also writes every out-of-memory partition attempt of the search as a MetisMiss, in no
+ * particular order (sort them with metis_sort_records).  The number of attempts lands in summary->reserved[3], also
+ * when it exceeds miss_capacity (then only the first miss_capacity are written: search again with more room).
+ *   misses [device] miss_capacity records, or NULL (then exactly metis_het_search_headroom)
+ */
+int metis_het_search_outputs(const MetisProblem *problem, const MetisPlanSpace *space, const MetisShard *shard,
+                             MetisRecord *records, int64_t capacity, uint8_t *detail, int32_t detail_stride,
+                             double *headroom, MetisMiss *misses, int64_t miss_capacity, void *workspace,
+                             int64_t workspace_bytes, MetisSearchSummary *summary, void *stream);
 
 /*
  * Re-evaluates the listed (ordinal, step) candidates and writes their strategies and

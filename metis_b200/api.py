@@ -176,6 +176,9 @@ class HetSearchResult(Sequence):
         # MB) over the stages of its accepted partition attempt; None unless searched with headroom=True
         self.headroom = getattr(candidates, 'headroom', None)
         self._headroom_index = None
+        self._misses = getattr(candidates, 'misses', None)   # MISS_HOST_DTYPE rows, or None without misses=True
+        self._misses_view = None
+        self._closest = None                  # positions of the misses by ascending deficit (device sort)
         self.rank_order = rank_order          # permutation of sorted(..., key=cost); computed on first use (``ranker``)
         self.summary = summary
         self.timings = timings or {}
@@ -245,6 +248,45 @@ class HetSearchResult(Sequence):
             self._headroom_index = search.HeadroomIndex(self.candidates.records, self.headroom, self._rank(),
                                                         getattr(self.candidates, 'device', None))
         return self._headroom_index
+
+    @property
+    def misses(self):
+        """Every out-of-memory partition attempt of the search (needs ``misses=True``): a search.Misses of numpy columns
+        ``ordinal`` (global, int64), ``call``, ``attempt``, ``stage`` and ``deficit`` (MB, > 0), in the order the
+        reference prints them: (ordinal, call, attempt)."""
+        if self._misses is None:
+            raise ValueError('this result has no misses: call cost_het_cluster(..., misses=True)')
+        if self._misses_view is None:
+            from . import search
+            self._misses_view = search.Misses(self._misses)
+        return self._misses_view
+
+    def _closest_order(self) -> np.ndarray:
+        if self._closest is None:
+            from . import search
+            self._closest = search.closest_order(self.misses.deficit, getattr(self.candidates, 'device', None))
+        return self._closest
+
+    def closest_misses(self, k: int) -> List[Tuple]:
+        """The ``k`` out-of-memory attempts with the smallest deficit (needs ``misses=True``), closest first, ties in
+        the reference's order (the device record sort): tuples (node_sequence, device_groups, strategies, batches,
+        layer_partition, attempt, deficit, stage).  The strategies and partition of each attempt come from replaying
+        its plan (metis_het_trace)."""
+        from . import search
+        misses = self.misses
+        if int(k) < 0:
+            raise ValueError(f'k must be >= 0, not {k}')
+        return search.miss_tuples(self.candidates, misses, self._closest_order()[:int(k)])
+
+    def miss_detail(self, idx):
+        """Per-stage performance (fed to the attempt's balancer run), memory capacity, demand and state of the misses
+        ``idx`` (an int, a slice or an index array of positions into ``misses``), NaN past a miss's stages
+        (search.MissDetail).  Replayed like closest_misses."""
+        from . import search
+        misses = self.misses
+        if isinstance(idx, slice):
+            idx = np.arange(len(misses))[idx]
+        return search.miss_detail(self.candidates, misses, idx)
 
     def pareto(self) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """The cost / headroom Pareto front (needs ``headroom=True``): (positions in estimate_costs order, their costs,
@@ -346,7 +388,7 @@ def release_engines() -> None:
 def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, model_config: ModelConfig,
                      cost_estimator: HeteroCostEstimator, layer_load_balancer: LayerLoadBalancer,
                      node_sequences: Optional[Sequence[Sequence]] = None, device=None,
-                     corrected: Sequence[str] = (), headroom: bool = False) -> HetSearchResult:
+                     corrected: Sequence[str] = (), headroom: bool = False, misses: bool = False) -> HetSearchResult:
     """cost_het_cluster.py:21-50 on the GPU.  Returns the same sequence of
     (node_sequence, device_groups, strategies, batches, layer_partition, num_repartition, cost) in the
     same order (see HetSearchResult).  With torch.distributed initialised the plans are sharded over the ranks and
@@ -362,7 +404,11 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
 
     ``headroom=True``: the search kernels also write every candidate's memory headroom (``result.headroom``), which
     ``result.ranked(k, min_headroom=...)`` and ``result.pareto()`` need; ``timings['headroom_s']`` is the host time spent
-    ordering and copying it."""
+    ordering and copying it.
+
+    ``misses=True``: the search kernels also write every out-of-memory partition attempt (``result.misses``), which
+    ``result.closest_misses(k)`` and ``result.miss_detail(idx)`` need; ``summary['num_oom_attempts']`` counts them and
+    ``timings['misses_s']`` is the host time spent ordering and copying them."""
     unknown = set(corrected) - {'Q1', 'Q2', 'Q5', 'Q6'}
     if unknown:
         raise ValueError(f'unknown corrections {sorted(unknown)}: choose from Q1, Q2, Q5, Q6')
@@ -387,7 +433,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
             space, windows = windows[0].space, None
     t1 = time.perf_counter()
     if windows is not None:
-        result = _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1, headroom)
+        result = _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1, headroom,
+                                   misses)
         result.summary['listing'] = 'host' if listing is None else 'device'
         return result
     stride = 3 * int(space.blocks['num_stage'].max()) + 1
@@ -395,6 +442,9 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     searcher.want_headroom = headroom
     if not headroom:
         searcher.headroom = None
+    searcher.want_misses = misses
+    if not misses:
+        searcher.misses, searcher.miss_capacity = None, 0
     dp.upload()
     failure = None
     out = best = None
@@ -416,6 +466,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
         else:
             summary['fatal_ordinal'] = 2 ** 64 - 1
             out = search.gather_records(out, searcher, want_rank=False, counts=summary['records_per_rank'])
+            if misses:
+                summary['num_oom_attempts'] = len(out.misses)
     else:
         summary, best = out.summary, out.best
     if summary['fatal_ordinal'] != 2 ** 64 - 1:
@@ -425,7 +477,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     # the row blob of the engine is rewritten by the next call: a lazy result keeps its own copy (a few MB, on the GPU)
     cand = search.Candidates(out.records, out.detail, space, seqs, detail_dev=out.detail_dev,
                              rows_dev=dp.rows_device().clone(), problem=problem,
-                             headroom=np.array(out.headroom) if headroom else None)
+                             headroom=np.array(out.headroom) if headroom else None,
+                             misses=out.misses if misses else None)   # a fresh array (HetSearcher.run)
     # sorted(result, key=cost) is the CALLER's step in the reference (cost_het_cluster.py:76): its permutation is
     # computed by the device sort when ranked() is first asked for; best() needs no sort at all
     result = HetSearchResult(cand, out.rank_order,
@@ -437,6 +490,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
                       'decode_columns_s': time.perf_counter() - t2}
     if headroom:
         result.timings['headroom_s'] = out.headroom_s
+    if misses:
+        result.timings['misses_s'] = out.misses_s
     return result
 
 
@@ -533,13 +588,14 @@ def _het_windows(problem, space, dev, rank: int, world: int, num_recs: Optional[
 
 
 def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int, dist, corrected, t0: float,
-                      t1: float, headroom: bool = False) -> HetSearchResult:
+                      t1: float, headroom: bool = False, misses: bool = False) -> HetSearchResult:
     """cost_het_cluster() for a space larger than one search: flatten.plan_windows' windows, searched in ordinal order
     (search.search_windows), merged on the host; the result keeps the records only (search.WindowedCandidates)."""
     from . import search
     failure = merged = searcher = None
     try:
-        merged, _dp, searcher = search.search_windows(problem, windows, dev, rank, world, headroom=headroom)
+        merged, _dp, searcher = search.search_windows(problem, windows, dev, rank, world, headroom=headroom,
+                                                      misses=misses)
     except Exception as exc:                                  # noqa: BLE001 - re-raised below on every rank
         if not dist:
             raise
@@ -555,13 +611,15 @@ def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int,
         else:
             summary['fatal_ordinal'] = 2 ** 64 - 1
             merged = search.gather_window_records(merged, dev)
+            if misses:
+                summary['num_oom_attempts'] = len(merged.misses)
     else:
         summary, best = merged.summary, merged.best
     if summary['fatal_ordinal'] != 2 ** 64 - 1:
         search.raise_fatal(summary, problem)                  # the reference dies at that plan (quirk Q8)
     t2 = time.perf_counter()
     cand = search.WindowedCandidates(merged.records, merged.bases, merged.firsts, windows, problem, seqs, searcher,
-                                     headroom=merged.headroom)
+                                     headroom=merged.headroom, misses=merged.misses)
     result = HetSearchResult(cand, None, dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)),
                                               num_windows=len(windows)),
                              best_key=(best[1], best[2]) if best else None)
@@ -571,6 +629,8 @@ def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int,
                       'decode_columns_s': time.perf_counter() - t2}
     if headroom:
         result.timings['headroom_s'] = merged.headroom_s
+    if misses:
+        result.timings['misses_s'] = merged.misses_s
     return result
 
 

@@ -833,7 +833,10 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
 
     // One attempt of LayerLoadBalancer.partition_layer after the balancer (model/load_balancer.py:127-143):
     // memory demand (:29-55), OOM test (:57-63), capacity re-weighting.  Returns like PlanEvaluator::memory_phase.
-    MB_HD int memory_phase_coop(int attempt) {
+    // A sink with misses (SinkMisses) gets the attempt when memory runs out, unless `report` is false (an attempt the
+    // bulk round already reported, CoopEvaluator::kReplay).
+    template <class Sink>
+    MB_HD int memory_phase_coop(int attempt, Sink &sink, bool report) {
         shared_scratch();
         const int S = pd.S;
         bool failed = false, oom = false;
@@ -855,6 +858,18 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
             METIS_PAR(x, s, S) w.mstate[s] = w.capa[s];
             x.sync();
             return 1;
+        }
+        if constexpr (SinkMisses<Sink>::value) {             // w.capa holds the states (w.mstate error codes)
+            if (report) {
+                double m = INFINITY;
+                int at = 0x7FFFFFFF;
+                METIS_PAR(x, s, S)
+                    if (w.capa[s] < m || (w.capa[s] == m && s < at)) { m = w.capa[s]; at = s; }
+                x.argmin_first(m, at);
+                sink.miss(pd, attempt, -m, at);              // the sink writes from the leader lane only
+            }
+        } else {
+            (void)sink, (void)report;
         }
         if (attempt >= 3) return 0;
         x.mark(21);
@@ -926,6 +941,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         bool started = false, have_state = false;
         bool skip_first = start == kReplay;
         int nrep = 0, step = 0;
+        int call = start == kAdvance ? 1 : 0;                 // partition_layer call of the plan (misses only)
         if (start == kRetry) {
             METIS_PAR(x, s, pd.S) w.perf[s] = perf[(size_t)s * perf_stride];
             x.sync();
@@ -943,6 +959,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                     if (start == kRetry) first_attempt = 2;
                 } else if (!next_strategy_coop(have_state)) return;   // :203-204
                 if (!this->valid()) continue;
+                miss_call(sink, call++);
                 int rc = 0;
                 if (first_attempt == 1) {
                     if (!skip_first) sink.partition_call();
@@ -953,13 +970,14 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                 attempt = 0;
 #pragma unroll 1
                 for (int a = first_attempt; a <= 3; ++a) {    // LayerLoadBalancer.partition_layer (:121-144)
-                    if (!skip_first) sink.balancer_run();
+                    const bool fresh = !skip_first;           // not an attempt the bulk round counted and reported
+                    if (fresh) sink.balancer_run();
                     skip_first = false;
                     x.gate(kGateRun, 9);                      // gate points (ChainCoop::gate): the block meets at the vote
                     rc = balance_coop();
                     if (rc) { sink.fatal(pd.ordinal, rc, aux); return; }
                     x.gate(kGateMemory, 20);
-                    const int r = memory_phase_coop(a);
+                    const int r = memory_phase_coop(a, sink, fresh);
                     if (r < 0) { sink.fatal(pd.ordinal, -r, aux); return; }
                     if (r == 1) { attempt = a; break; }
                     if (r == 0) break;

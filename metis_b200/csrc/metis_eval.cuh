@@ -839,6 +839,21 @@ MB_HD_NOINLINE int partition_data(const Tables &T, int ns, int rank_lo, int coun
 //   void partition_call(); void balancer_run(); void keyerror(); void phase(int) (profiling hook);
 //   void fatal(uint32_t ordinal, int code, uint32_t aux);
 //   void emit(const PlanDesc&, int step, int nrep, double cost, const uint8_t *tpc, const uint16_t *part);
+// A sink that declares `static constexpr bool kMisses = true` also gets every out-of-memory partition attempt
+// (metis_het_search_outputs): the evaluators set its `int call` (0-based partition_layer call of the plan) when a
+// call starts and then call
+//   void miss(const PlanDesc&, int attempt, double deficit, int stage);
+// after the attempt's memory_state is known and before the re-weighting overwrites it: deficit = -min_s state[s] > 0,
+// stage = the lowest s attaining that minimum.  Every other sink compiles without a trace of it.
+template <class Sink, class = void>
+struct SinkMisses { static constexpr bool value = false; };
+template <class Sink>
+struct SinkMisses<Sink, decltype(void(Sink::kMisses))> { static constexpr bool value = Sink::kMisses; };
+template <class Sink>
+MB_HD void miss_call(Sink &sink, int call) {
+    if constexpr (SinkMisses<Sink>::value) sink.call = call;
+    else (void)sink, (void)call;
+}
 
 // Optional tap of intermediate values for the verbose transcript and the cost breakdown (metis_trace.cuh); null in
 // the search kernels.  homo_cost fills `demand` (per-stage memory sums, cost_estimator.py:121-122) and `cost` only.
@@ -1283,8 +1298,14 @@ struct PlanEvaluator {
     // capacity re-weighting.  returns 1 = partition accepted (w.mstate = memory_state), 2 = retry
     // with the adjusted w.perf, 0 = (None, -1, None), <0 = fatal (negated code).  After the third
     // failed attempt the reference still evaluates _adj_compute_performance and discards it; that
-    // call is skipped here.
+    // call is skipped here.  A sink with misses (SinkMisses) gets the attempt when memory runs out.
+    struct NoMisses {};
     MB_HD int memory_phase(int attempt) {
+        NoMisses none;
+        return memory_phase(attempt, none);
+    }
+    template <class Sink>
+    MB_HD int memory_phase(int attempt, Sink &sink) {
         const int S = pd.S;
         bool oom = false;
         int rc = 0;
@@ -1301,6 +1322,16 @@ struct PlanEvaluator {
         x.converge();
         if (rc) return -rc;
         if (!oom) return 1;
+        if constexpr (SinkMisses<Sink>::value) {             // every stage's state is in w.mstate
+            double m = w.mstate[0];
+            int at = 0;
+#pragma unroll 1
+            for (int s = 1; s < S; ++s)
+                if (w.mstate[s] < m) { m = w.mstate[s]; at = s; }
+            sink.miss(pd, attempt, -m, at);
+        } else {
+            (void)sink;
+        }
         if (attempt >= 3) return 0;
         x.mark(21);
         const int adj = adjust_performance();
@@ -1317,7 +1348,7 @@ struct PlanEvaluator {
             sink.balancer_run();
             const int rc = balance_run<MAXS, MAXL>(T, pd.S, w, x);
             if (rc) return -rc;
-            const int r = memory_phase(attempt);
+            const int r = memory_phase(attempt, sink);
             if (r == 1) return attempt;
             if (r <= 0) return r;
         }
@@ -1472,7 +1503,7 @@ struct PlanEvaluator {
         if (ok < 0) { sink.fatal(plan.ordinal, METIS_FATAL_SCRATCH, 0); return; }
         if (ok == 0) return;
         bool started = false, have_state = false;
-        int nrep = 0, step = 0;
+        int nrep = 0, step = 0, call = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (;;) {
             if (nrep == 1) return;                            // plan.py:194-195
@@ -1482,6 +1513,7 @@ struct PlanEvaluator {
                 if (!started) started = true;                 // first strategy that can be valid (see begin)
                 else if (!next_strategy(have_state)) return;  // :203-204
                 if (!valid()) continue;
+                miss_call(sink, call++);
                 sink.partition_call();
                 int rc = compute_performance();
                 if (rc) { sink.fatal(pd.ordinal, rc, aux); return; }
@@ -1529,6 +1561,7 @@ MB_HD bool first_task(const Tables &T, Scratch<MAXS, MAXL> &w, Sink &sink, bool 
     }
     ev.x.rejoin(has);
     if (has) {
+        miss_call(sink, 0);
         sink.partition_call();
         const int rc = ev.compute_performance();
         if (rc) { sink.fatal(plan.ordinal, rc, ev.aux); has = false; }
@@ -1544,7 +1577,7 @@ MB_HD bool first_task(const Tables &T, Scratch<MAXS, MAXL> &w, Sink &sink, bool 
     ev.x.rejoin(has);
     bool costing = false;
     if (has) {                                               // ---- M ----
-        const int r = ev.memory_phase(1);
+        const int r = ev.memory_phase(1, sink);           // reports attempt 1 of call 0 when it runs out of memory
         if (r < 0) sink.fatal(plan.ordinal, -r, ev.aux);
         else if (r != 1) {                                   // out of memory: the rest in the chain kernel
             cont = true;

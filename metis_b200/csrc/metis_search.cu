@@ -24,6 +24,8 @@
 //   homo_breakdown_kernel the same with the cost terms and per-stage memory
 //   layer_balance_kernel  a10 alone, for unit parity
 //   (rank_records_kernel, the stable record sort, lives in metis_rank.cu; the headroom select / front in metis_select.cu)
+//   het_first_kernel and het_chain_kernel are compiled per output mask OUT (kOutHeadroom | kOutMisses): the side
+//   outputs of metis_het_search_outputs exist only in the instantiations that write them
 //
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (no FMA contraction: parity).
 #include <cuda_runtime.h>
@@ -282,6 +284,7 @@ struct DeviceOut {
     uint8_t *detail;
     int detail_stride;
     unsigned long long *counters;   // [0] records [1] partition calls [2] balancer runs [3] keyerrors [4] fatal key
+                                    // [5] out-of-memory partition attempts (MissSink)
     MetisRecord *block_best;
 };
 
@@ -356,8 +359,50 @@ struct HeadroomSink : DeviceSink {
         });
     }
 };
-template <bool HEAD>
-using SearchSink = typename std::conditional<HEAD, HeadroomSink, DeviceSink>::type;
+
+// Where the misses of a search go: misses[0, capacity), counted on counters[5] (DeviceOut)
+struct MissOut {
+    MetisMiss *misses;
+    long long capacity;
+};
+
+// Sink of the search kernels compiled with misses (output bit kOutMisses): `Base`'s, and every out-of-memory partition
+// attempt as a 16-byte MetisMiss, one atomic on its own counter.  The count is exact past the capacity.
+// The key `call << 2 | attempt` has 14 bits for the call.  A plan makes at most S * floor(log2(max_tp)) + 1 calls:
+// every strategy of its chain doubles one stage's tp (plan.py:257-266), tp never shrinks, and a call is made only for a
+// valid strategy, whose every tp is <= max_tp (:238-249).  With S <= METIS_MAX_STAGES and max_tp < 2^31 that is below
+// 2^14, so the key cannot wrap.
+static_assert(METIS_MAX_STAGES * 30 + 1 < (1 << 14), "MetisMiss.key: call index may not fit in 14 bits");
+template <class Base>
+struct MissSink : Base {
+    static constexpr bool kMisses = true;
+    MissOut mo;
+    int call;                       // partition_layer call of the current plan (set by the evaluators)
+    __device__ MissSink(const DeviceOut &out, double *h, const MissOut &m) : Base(out, h), mo(m), call(0) {}
+    __device__ void miss(const PlanDesc &pd, int attempt, double deficit, int stage) {
+        if (!this->leader) return;
+        const unsigned long long slot = atomicAdd(&this->o.counters[5], 1ULL);
+        if ((long long)slot < mo.capacity) {
+            MetisMiss r;
+            r.deficit = deficit; r.ordinal = pd.ordinal; r.key = (uint16_t)((call << 2) | attempt);
+            r.stage = (uint8_t)stage; r.num_stage = (uint8_t)pd.S;
+            mo.misses[slot] = r;
+        }
+    }
+};
+
+// the side outputs of a search kernel instantiation (template argument OUT): a mask of these bits
+constexpr int kOutHeadroom = 1, kOutMisses = 2;
+template <int OUT>
+struct SinkOf {
+    using Plain = typename std::conditional<(OUT & kOutHeadroom) != 0, HeadroomSink, DeviceSink>::type;
+    using type = typename std::conditional<(OUT & kOutMisses) != 0, MissSink<Plain>, Plain>::type;
+};
+template <int OUT, class S = typename SinkOf<OUT>::type>
+__device__ __forceinline__ S make_sink(const DeviceOut &out, double *headroom, const MissOut &m) {
+    if constexpr ((OUT & kOutMisses) != 0) return S(out, headroom, m);
+    else return S(out, headroom);
+}
 
 // End of a search kernel: counters (warp reduce, one atomic per warp) and the block's best candidate:
 // argmin (cost, ordinal, step) by __shfl_xor_sync inside the warp, then across the warps through shared memory.
@@ -511,20 +556,21 @@ het_scatter_kernel(const SearchLists ls) {
     }
 }
 
-template <int MAXS, int MAXL, bool ONE, bool HEAD>
+template <int MAXS, int MAXL, bool ONE, int OUT>
 __global__ void __launch_bounds__(kThreads, (MAXS <= 64 ? METIS_MIN_BLOCKS : ONE ? METIS_MIN_BLOCKS_BIG_ONE : METIS_MIN_BLOCKS_BIG))
 het_first_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ MetisPlanSpace sp,
                  const __grid_constant__ BlobLayout lay, const uint8_t *__restrict__ blob, const int use_smem,
-                 const __grid_constant__ DeviceOut out, const SearchLists ls, const int best_slot, double *headroom) {
+                 const __grid_constant__ DeviceOut out, const SearchLists ls, const int best_slot, double *headroom,
+                 const MissOut misses) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
     __shared__ Tables s_tables;
-    SearchSink<HEAD> sink(out, headroom);
+    auto sink = make_sink<OUT>(out, headroom, misses);
     const unsigned int n = ls.ctl[0];
     if ((long long)n >= ls.bulk_min) {
         const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
         Scratch<MAXS, MAXL> w;
-        if constexpr (HEAD) sink.state = w.mstate;
+        if constexpr ((OUT & kOutHeadroom) != 0) sink.state = w.mstate;
         const int lane = threadIdx.x & 31;
         for (;;) {                                           // batches of 32 plans, longest stage counts first
             unsigned int fetched = 0;
@@ -592,22 +638,22 @@ struct alignas(16) ChainScratch {
 
 
 // 64 registers per thread: 32 resident warps per SM in blocks of 16 warps (tables staged once per block)
-template <int MAXS, int MAXL, bool ONE, bool HEAD>
+template <int MAXS, int MAXL, bool ONE, int OUT>
 __global__ void __launch_bounds__(512, 2)
 het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ MetisPlanSpace sp,
                  const __grid_constant__ BlobLayout lay, const uint8_t *__restrict__ blob, const int use_smem,
                  const unsigned int scratch_off, const __grid_constant__ DeviceOut out, const SearchLists ls,
-                 const int best_slot, double *headroom) {
+                 const int best_slot, double *headroom, const MissOut misses) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
     __shared__ Tables s_tables;
     WarpCoop::prof_init();                                   // (phase clock build only; published by block_tables)
     const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
-    SearchSink<HEAD> sink(out, headroom);
+    auto sink = make_sink<OUT>(out, headroom, misses);
     const int lane = threadIdx.x & 31;
     sink.leader = lane == 0;
     ChainScratch<MAXS, MAXL> *cs = reinterpret_cast<ChainScratch<MAXS, MAXL> *>(smem + scratch_off) + (threadIdx.x >> 5);
-    if constexpr (HEAD) sink.state = cs->w.mstate;           // read by the leader after run_chain's x.sync()
+    if constexpr ((OUT & kOutHeadroom) != 0) sink.state = cs->w.mstate;           // read by the leader after run_chain's x.sync()
     const unsigned int n_adm = ls.ctl[0];
     const bool bulk = (long long)n_adm >= ls.bulk_min;
     const uint4 *list = ls.b;                                // sorted: by chain hint after a bulk round, else by stage count
@@ -678,6 +724,7 @@ __global__ void het_finalize_kernel(const MetisRecord *block_best, int nblocks, 
         s.reserved[0] = ctl[0];                                          // plans admitted
         s.reserved[1] = ctl[2];                                          // plans handed to the chain kernel by the bulk round
         s.reserved[2] = instantiation;                                   // MAXS | MAXL << 16 | ONE << 32 of the kernels
+        s.reserved[3] = counters[5];                                     // out-of-memory partition attempts (misses)
         *summary = s;
     }
 }
@@ -949,10 +996,10 @@ static Workspace carve(void *ws, const BlobLayout &lay) {
 }  // extern "C"
 
 // Launch configuration of one search: which instantiation, how the tables are staged, block shapes.
-template <int MAXS, int MAXL, bool ONE, bool HEAD>
+template <int MAXS, int MAXL, bool ONE, int OUT>
 static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg, const MetisShard &sh,
                          const BlobLayout &lay, const Workspace &ws, const DeviceOut &out, double *headroom,
-                         int64_t slots, cudaStream_t stream) {
+                         const MissOut &misses, int64_t slots, cudaStream_t stream) {
     cudaError_t e;
     int dev = 0, sms = 0, smem_optin = 0;
     cudaGetDevice(&dev);
@@ -972,7 +1019,7 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     ls.save_cap = (unsigned int)save_slots(cap);
 
     // ---- chain kernel: warps per block chosen so that tables + per-warp scratch fill the SM with warps ----
-    auto chain = het_chain_kernel<MAXS, MAXL, ONE, HEAD>;
+    auto chain = het_chain_kernel<MAXS, MAXL, ONE, OUT>;
     const size_t per_warp = sizeof(ChainScratch<MAXS, MAXL>);
     int chain_smem_tables = (int)lay.total <= blob_max;
     int chain_threads = 0, chain_per_sm = 0;
@@ -1003,7 +1050,7 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     int64_t chain_grid = (int64_t)sms * chain_per_sm;
 
     // ---- bulk round ----
-    auto first = het_first_kernel<MAXS, MAXL, ONE, HEAD>;
+    auto first = het_first_kernel<MAXS, MAXL, ONE, OUT>;
     int first_smem_tables = (int)lay.total <= blob_max && blob_pad <= (unsigned int)smem_optin;
     size_t first_dyn = first_smem_tables ? blob_pad : 0;
     e = cudaFuncSetAttribute(first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_dyn);
@@ -1027,10 +1074,11 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
         if (scatter_blocks > 8LL * sms) scatter_blocks = 8LL * sms;
         het_scatter_kernel<<<(unsigned)scatter_blocks, 256, 0, stream>>>(ls);
         first<<<(unsigned)first_grid, kThreads, first_dyn, stream>>>(p_arg, s_arg, lay, ws.blob, first_smem_tables, out, ls, 0,
-                                                                  headroom);
+                                                                  headroom, misses);
         het_order_kernel<<<(unsigned)(2 * sms), 256, 0, stream>>>(ls);
         chain<<<(unsigned)chain_grid, chain_threads, chain_dyn, stream>>>(p_arg, s_arg, lay, ws.blob, chain_smem_tables,
-                                                                         chain_off, out, ls, (int)first_grid, headroom);
+                                                                         chain_off, out, ls, (int)first_grid, headroom,
+                                                                         misses);
         e = cudaGetLastError();
         if (e != cudaSuccess) return cuda_fail(e, "search kernels");
     }
@@ -1048,18 +1096,19 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
 // three instantiations: per-warp scratch of the chain kernel (and per-thread scratch of the bulk round)
 // sized for S <= 64 / L <= 128, S <= 96 / L <= 128, and the compiled limits
 // ... each once for single-type clusters (no mixed-type code at all) and once for the general case
-template <bool HEAD>
+template <int OUT>
 static int launch_tier(const MetisProblem &p, const MetisPlanSpace &sp, const MetisShard &sh, const BlobLayout &lay,
-                       const Workspace &ws, const DeviceOut &out, double *headroom, int64_t slots, cudaStream_t stream) {
+                       const Workspace &ws, const DeviceOut &out, double *headroom, const MissOut &m, int64_t slots,
+                       cudaStream_t stream) {
     const bool one = p.num_types == 1;
     if (sp.max_stage <= 64 && p.num_layers <= 128)
-        return one ? launch_search<64, 128, true, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream)
-                   : launch_search<64, 128, false, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream);
+        return one ? launch_search<64, 128, true, OUT>(p, sp, sh, lay, ws, out, headroom, m, slots, stream)
+                   : launch_search<64, 128, false, OUT>(p, sp, sh, lay, ws, out, headroom, m, slots, stream);
     if (sp.max_stage <= 96 && p.num_layers <= 128)
-        return one ? launch_search<96, 128, true, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream)
-                   : launch_search<96, 128, false, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream);
-    return one ? launch_search<kMaxS, kMaxL, true, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream)
-               : launch_search<kMaxS, kMaxL, false, HEAD>(p, sp, sh, lay, ws, out, headroom, slots, stream);
+        return one ? launch_search<96, 128, true, OUT>(p, sp, sh, lay, ws, out, headroom, m, slots, stream)
+                   : launch_search<96, 128, false, OUT>(p, sp, sh, lay, ws, out, headroom, m, slots, stream);
+    return one ? launch_search<kMaxS, kMaxL, true, OUT>(p, sp, sh, lay, ws, out, headroom, m, slots, stream)
+               : launch_search<kMaxS, kMaxL, false, OUT>(p, sp, sh, lay, ws, out, headroom, m, slots, stream);
 }
 
 extern "C" {
@@ -1075,6 +1124,14 @@ int metis_het_search_headroom(const MetisProblem *problem, const MetisPlanSpace 
                               MetisRecord *records, int64_t capacity, uint8_t *detail, int32_t detail_stride,
                               double *headroom, void *workspace, int64_t workspace_bytes, MetisSearchSummary *summary,
                               void *stream_) {
+    return metis_het_search_outputs(problem, space, shard, records, capacity, detail, detail_stride, headroom, nullptr, 0,
+                                    workspace, workspace_bytes, summary, stream_);
+}
+
+int metis_het_search_outputs(const MetisProblem *problem, const MetisPlanSpace *space, const MetisShard *shard,
+                             MetisRecord *records, int64_t capacity, uint8_t *detail, int32_t detail_stride,
+                             double *headroom, MetisMiss *misses, int64_t miss_capacity, void *workspace,
+                             int64_t workspace_bytes, MetisSearchSummary *summary, void *stream_) {
     int rc = check_problem(problem);
     if (rc) return rc;
     if (!space || !shard || !workspace || !summary) return arg_fail("NULL argument");
@@ -1090,6 +1147,7 @@ int metis_het_search_headroom(const MetisProblem *problem, const MetisPlanSpace 
     if (detail && detail_stride < 3 * space->max_stage + 1) return arg_fail("detail_stride too small (3 * max_stage + 1)");
     if (capacity < 0 || (capacity > 0 && !records)) return arg_fail("records/capacity mismatch");
     if (headroom && !records) return arg_fail("headroom without records");
+    if (miss_capacity < 0 || (miss_capacity > 0 && !misses)) return arg_fail("misses/miss_capacity mismatch");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const BlobLayout lay = make_layout(*problem);
     const int64_t slots = shard_plan_slots(space->num_plans, shard);
@@ -1113,8 +1171,16 @@ int metis_het_search_headroom(const MetisProblem *problem, const MetisPlanSpace 
     DeviceOut out;
     out.records = records; out.capacity = capacity; out.detail = detail; out.detail_stride = detail_stride;
     out.counters = ws.counters; out.block_best = ws.block_best;
-    rc = headroom ? launch_tier<true>(*problem, *space, *shard, lay, ws, out, headroom, slots, stream)
-                  : launch_tier<false>(*problem, *space, *shard, lay, ws, out, nullptr, slots, stream);
+    // only the outputs asked for are compiled into the kernels that run: without them, exactly the plain search
+    MissOut mo;
+    mo.misses = misses; mo.capacity = misses ? miss_capacity : 0;
+    const int outs = (headroom ? kOutHeadroom : 0) | (misses ? kOutMisses : 0);
+    switch (outs) {
+    case 0: rc = launch_tier<0>(*problem, *space, *shard, lay, ws, out, nullptr, mo, slots, stream); break;
+    case kOutHeadroom: rc = launch_tier<kOutHeadroom>(*problem, *space, *shard, lay, ws, out, headroom, mo, slots, stream); break;
+    case kOutMisses: rc = launch_tier<kOutMisses>(*problem, *space, *shard, lay, ws, out, nullptr, mo, slots, stream); break;
+    default: rc = launch_tier<kOutHeadroom | kOutMisses>(*problem, *space, *shard, lay, ws, out, headroom, mo, slots, stream);
+    }
     if (rc) return rc;
     e = cudaMemcpyAsync(summary, ws.summary, sizeof(MetisSearchSummary), cudaMemcpyDeviceToHost, stream);
     if (e != cudaSuccess) return cuda_fail(e, "copy summary");

@@ -85,6 +85,7 @@ COMP_DTYPE = [('row_offset', '<i8'), ('pool_offset', '<u4'), ('stages', '<u2'), 
 RANGE_DTYPE = [('stages', '<i4'), ('reserved', '<i4'), ('first_row', '<i8'), ('end_row', '<i8')]   # MetisRowRange
 BREAKDOWN_DTYPE = [('terms', '<f8', (6,)), ('min_headroom', '<f8'), ('min_stage', '<i2'), ('costed_stages', '<i2'),
                    ('num_stage', '<i2'), ('reserved', '<i2')]                                     # MetisBreakdown
+MISS_DTYPE = [('deficit', '<f8'), ('ordinal', '<u4'), ('key', '<u2'), ('stage', 'u1'), ('num_stage', 'u1')]   # MetisMiss
 BD_FIELDS = 8                                  # METIS_BD_FIELDS: per-stage fields of metis_het_breakdown's stage_out
 
 SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 'metis_het_workspace_bytes', 'metis_het_search',
@@ -93,7 +94,7 @@ SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 
            'metis_enum_device_group_tables', 'metis_sort_workspace_bytes', 'metis_sort_records',
            'metis_enum_compositions', 'metis_generate_rows', 'metis_list_workspace_bytes', 'metis_list_stages',
            'metis_list_window', 'metis_het_search_headroom', 'metis_headroom_workspace_bytes', 'metis_headroom_select',
-           'metis_headroom_front']
+           'metis_headroom_front', 'metis_het_search_outputs']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -127,6 +128,10 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_het_search_headroom.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisShard),
                                               C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                               C.c_int64, C.c_void_p, C.c_void_p]
+    lib.metis_het_search_outputs.restype = C.c_int
+    lib.metis_het_search_outputs.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisShard),
+                                             C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                             C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.metis_headroom_workspace_bytes.restype = C.c_int64
     lib.metis_headroom_workspace_bytes.argtypes = [C.c_int64]
     lib.metis_headroom_select.restype = C.c_int

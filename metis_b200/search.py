@@ -171,6 +171,45 @@ class HetSearchOutput:
     headroom: Optional[np.ndarray] = None                 # float64 [n] aligned with records (want_headroom)
     headroom_dev: Optional[torch.Tensor] = None           # the same on the device
     headroom_s: float = 0.0                               # host time spent ordering and copying the headroom
+    misses: Optional[np.ndarray] = None                   # MISS_HOST_DTYPE in reference order (want_misses)
+    misses_s: float = 0.0                                 # host time spent ordering and copying the misses
+
+
+# Host form of the out-of-memory partition attempts of a search (native.MISS_DTYPE with a global 64-bit ordinal and the
+# key split): three 64-bit words without padding, so that a padded int64 tensor carries it through the multi-rank gathers
+# and the conversion below is word arithmetic.
+MISS_HOST_DTYPE = np.dtype([('deficit', '<f8'), ('ordinal', '<i8'), ('call', '<u2'), ('attempt', 'u1'), ('stage', 'u1'),
+                            ('num_stage', '<u4')])
+
+
+def misses_to_host(raw: np.ndarray, base: int = 0) -> np.ndarray:
+    """native.MISS_DTYPE rows (ordinals relative to ``base``) -> MISS_HOST_DTYPE rows, same order."""
+    words = np.ascontiguousarray(raw).view(np.uint64).reshape(-1, 2)
+    hi = words[:, 1]                                         # ordinal | key << 32 | stage << 48 | num_stage << 56
+    out = np.empty((len(raw), 3), dtype=np.uint64)
+    out[:, 0] = words[:, 0]
+    out[:, 1] = (hi & np.uint64(0xFFFFFFFF)) + np.uint64(base)
+    key = (hi >> np.uint64(32)) & np.uint64(0xFFFF)
+    out[:, 2] = ((key >> np.uint64(2)) | ((key & np.uint64(3)) << np.uint64(16)) |
+                 (((hi >> np.uint64(48)) & np.uint64(0xFF)) << np.uint64(24)) | ((hi >> np.uint64(56)) << np.uint64(32)))
+    return out.view(MISS_HOST_DTYPE).reshape(-1)
+
+
+def host_rows_device(words: torch.Tensor) -> torch.Tensor:
+    """misses_to_host on the device, base 0: int64 [2m] MetisMiss words -> int64 [m, 3] MISS_HOST_DTYPE words."""
+    w = words.view(-1, 2)
+    hi = w[:, 1]
+    key = (hi >> 32) & 0xFFFF
+    out = torch.empty((w.shape[0], 3), dtype=torch.int64, device=words.device)
+    out[:, 0] = w[:, 0]
+    out[:, 1] = hi & 0xFFFFFFFF
+    out[:, 2] = (key >> 2) | ((key & 3) << 16) | (((hi >> 48) & 0xFF) << 24) | (((hi >> 56) & 0xFF) << 32)
+    return out
+
+
+def position_order(misses: np.ndarray) -> np.ndarray:
+    """The reference's order of MISS_HOST_DTYPE rows: (ordinal, call, attempt)."""
+    return misses[np.lexsort((misses['attempt'], misses['call'], misses['ordinal']))]
 
 
 class HetSearcher:
@@ -179,9 +218,13 @@ class HetSearcher:
     def __init__(self, dp: DeviceProblem, rank: int = 0, world: int = 1, tile: int = 128,
                  want_records: bool = True, want_detail: bool = False, capacity: Optional[int] = None,
                  want_ranking: bool = False, detail_to_host: bool = True, detail_stride: Optional[int] = None,
-                 want_headroom: bool = False):
-        """``want_headroom``: the search also writes each record's memory headroom (metis_het_search_headroom)."""
+                 want_headroom: bool = False, want_misses: bool = False):
+        """``want_headroom``: the search also writes each record's memory headroom (metis_het_search_headroom).
+        ``want_misses``: and every out-of-memory partition attempt (metis_het_search_outputs)."""
         self.dp = dp
+        self.want_misses = want_misses
+        self.misses = None                                   # int64 [2 * miss_capacity]: MetisMiss rows
+        self.miss_capacity = 0
         self.want_headroom = want_headroom and want_records
         self.headroom = None
         self.want_ranking = want_ranking and want_records
@@ -231,10 +274,17 @@ class HetSearcher:
             self.detail = (torch.empty((capacity, self.detail_stride), dtype=torch.uint8, device=dev)
                            if self.want_detail else None)
 
+    def _alloc_misses(self, capacity: int) -> None:
+        self.miss_capacity = capacity
+        with torch.cuda.device(self.dp.device):
+            self.misses = torch.empty(capacity * 2, dtype=torch.int64, device=self.dp.device)
+
     def launch(self, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Enqueue pack + search + finalize + summary copy on ``stream`` (asynchronous)."""
         dp = self.dp
         s = stream or torch.cuda.current_stream(dp.device)
+        if self.want_misses and self.misses is None:         # the count is not known before the first search
+            self._alloc_misses(min(self.shard_plans + 4096, 1 << 18))
         if self.want_headroom and self.records is not None and self.headroom is None:
             with torch.cuda.device(dp.device):
                 self.headroom = torch.empty(self.capacity, dtype=torch.float64, device=dp.device)
@@ -242,7 +292,13 @@ class HetSearcher:
                   C.c_void_p(self.detail.data_ptr() if self.detail is not None else 0), C.c_int32(self.detail_stride))
         tail = (C.c_void_p(self.workspace.data_ptr()), C.c_int64(self.workspace.numel()),
                 C.c_void_p(self.summary_host.data_ptr()), C.c_void_p(s.cuda_stream))
-        if self.want_headroom:
+        if self.want_misses:
+            rc = dp.lib.metis_het_search_outputs(
+                C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard), *common,
+                C.c_void_p(self.headroom.data_ptr() if self.want_headroom else 0), C.c_void_p(self.misses.data_ptr()),
+                C.c_int64(self.miss_capacity), *tail)
+            native.check(rc, 'metis_het_search_outputs')
+        elif self.want_headroom:
             rc = dp.lib.metis_het_search_headroom(C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard),
                                                   *common, C.c_void_p(self.headroom.data_ptr()), *tail)
             native.check(rc, 'metis_het_search_headroom')
@@ -287,9 +343,13 @@ class HetSearcher:
             self.launch(s)
             s.synchronize()
             sm = self.summary()
-            if self.want_records and sm.num_records > self.capacity:
+            grow_misses = self.want_misses and sm.reserved[3] > self.miss_capacity
+            if (self.want_records and sm.num_records > self.capacity) or grow_misses:
                 # C is not known before the first search of a space: size the buffers and search again
-                self._alloc(int(sm.num_records) + max(1024, int(sm.num_records) // 64))
+                if self.want_records and sm.num_records > self.capacity:
+                    self._alloc(int(sm.num_records) + max(1024, int(sm.num_records) // 64))
+                if grow_misses:
+                    self._alloc_misses(int(sm.reserved[3]) + max(1024, int(sm.reserved[3]) // 64))
                 self.launch(s)
                 s.synchronize()
                 sm = self.summary()
@@ -304,8 +364,18 @@ class HetSearcher:
             if sm.num_records > 0:
                 b = sm.best
                 best = (float(b.cost), int(b.ordinal), int(b.step), int(b.num_repartition), int(b.num_stage))
-            records = detail = rank_order = detail_dev = records_dev = headroom = headroom_dev = None
-            headroom_s = 0.0
+            records = detail = rank_order = detail_dev = records_dev = headroom = headroom_dev = misses = None
+            headroom_s = misses_s = 0.0
+            if self.want_misses:                              # reference order: the record sort's position mode
+                t = time.perf_counter()
+                m = int(sm.reserved[3])
+                out_summary['num_oom_attempts'] = m
+                self.sort_records(m, native.SORT_POSITION, s, buf=self.misses)
+                with torch.cuda.stream(s):
+                    rows = host_rows_device(self.misses[:2 * m])
+                # a copy of plain words: the pinned buffer is reused by the next search, the result keeps the rows
+                misses = self._to_host('misses', rows, s).view(np.uint64).copy().view(MISS_HOST_DTYPE).reshape(-1)
+                misses_s = time.perf_counter() - t
             d2h = C.sizeof(native.MetisSearchSummary)
             if self.want_records:
                 n = int(sm.num_records)
@@ -332,7 +402,7 @@ class HetSearcher:
                     rank_order = self._to_host('rank', perm, s).view(np.uint32)
                     d2h += n * 4
         return HetSearchOutput(out_summary, best, records, detail, d2h, rank_order, detail_dev, records_dev, headroom,
-                               headroom_dev, headroom_s)
+                               headroom_dev, headroom_s, misses, misses_s)
 
     def sort_records(self, n: int, mode: int, stream: torch.cuda.Stream, want_perm: bool = False, buf=None):
         """metis_sort_records on the first n records (device, in place, asynchronous on ``stream``); returns the
@@ -397,8 +467,9 @@ class Candidates:
     def __init__(self, records: np.ndarray, detail: Optional[np.ndarray], space: flatten.FlatPlanSpace,
                  node_sequences: Sequence[Tuple], detail_dev: Optional[torch.Tensor] = None,
                  rows_dev: Optional[torch.Tensor] = None, problem: Optional[flatten.FlatProblem] = None,
-                 headroom: Optional[np.ndarray] = None):
+                 headroom: Optional[np.ndarray] = None, misses: Optional[np.ndarray] = None):
         self.records = records
+        self.misses = misses                  # MISS_HOST_DTYPE in reference order (a search with misses), else None
         self.headroom = headroom              # float64 per record (a search with headroom), else None
         self.device = rows_dev.device if rows_dev is not None else None   # where the search ran (None: not known)
         self.space = space
@@ -414,17 +485,7 @@ class Candidates:
     def columns(self, idx=None) -> Dict[str, np.ndarray]:
         """ns_idx, num_stage, row (dg_idx), batches, num_repartition of the candidates ``idx`` (default: all)."""
         rec = self.records if idx is None else self.records[idx]
-        blocks = self.space.blocks
-        ordinal = rec['ordinal'].astype(np.int64)
-        blk = (np.searchsorted(blocks['first_ordinal'], ordinal, side='right') - 1) if len(rec) \
-            else np.zeros(0, dtype=np.int64)
-        rel = ordinal - blocks['first_ordinal'][blk]
-        ndiv = len(self.space.batches)
-        row, stages = rel // ndiv, blocks['num_stage'][blk].astype(np.int64)
-        return dict(row=row, batches=self.space.batches[rel % ndiv].astype(np.int64),
-                    ns_idx=blocks['ns_idx'][blk].astype(np.int64), num_stage=stages,
-                    row_byte=blocks['rows_offset'][blk].astype(np.int64) + row * stages,
-                    num_repartition=rec['num_repartition'].astype(np.int64))
+        return dict(plan_geometry(self.space, rec['ordinal']), num_repartition=rec['num_repartition'].astype(np.int64))
 
     def group_codes(self, row_byte: np.ndarray, stages: np.ndarray) -> np.ndarray:
         """log2(device count) of every stage, uint8 [n, max stages] (columns past a row's stage count are junk)."""
@@ -450,9 +511,17 @@ class Candidates:
         """Cost terms and memory headroom of the candidates ``idx`` (metis_het_breakdown).  The problem tables and plan
         space descriptors are uploaded from this object's own copies, so a later search cannot change what is
         replayed."""
-        if self.problem is None:
-            raise ValueError('these candidates were built without their problem tables: no breakdown')
         idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        lib, p, sp, ws, dev, _keep = self._bound()
+        with torch.cuda.device(dev):
+            raw, stages = het_breakdown(lib, p, sp, ws, self.records[idx], dev, per_stage)
+        return Breakdown.from_raw(raw, stages)
+
+    def _bound(self):
+        """This object's problem tables and plan space on the device: (lib, problem struct, space struct, workspace,
+        device, the tensors the structs point into)."""
+        if self.problem is None:
+            raise ValueError('these candidates were built without their problem tables: no replay')
         dev = self._rows_dev.device if self._rows_dev is not None else _require_cuda(None)
         lib = native.load_library()
         with torch.cuda.device(dev):
@@ -465,8 +534,18 @@ class Candidates:
             p = self.problem.as_struct(lambda n: tens[n].data_ptr())
             sp = self.space.as_struct(lambda n: tens[n].data_ptr())
             ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=dev)
-            raw, stages = het_breakdown(lib, p, sp, ws, self.records[idx], dev, per_stage)
-        return Breakdown.from_raw(raw, stages)
+        return lib, p, sp, ws, dev, tens
+
+    def plan_columns(self, ordinals: np.ndarray) -> Dict[str, np.ndarray]:
+        """ns_idx, num_stage, batches and the log2 device-group codes of the plans ``ordinals``."""
+        col = plan_geometry(self.space, ordinals)
+        col['codes'] = self.group_codes(col['row_byte'], col['num_stage']) if len(ordinals) else np.zeros((0, 1), np.uint8)
+        return col
+
+    def trace(self, ordinals: np.ndarray) -> List[list]:
+        """verbose.decode_plan of the plans ``ordinals`` (metis_het_trace on this object's own tables)."""
+        lib, p, sp, ws, dev, _keep = self._bound()
+        return trace_decoded(lib, p, sp, ws, dev, ordinals, int(self.space.blocks['num_stage'].max()))
 
     def detail_rows(self, idx: np.ndarray) -> np.ndarray:
         if self._detail is None:
@@ -500,6 +579,52 @@ class Candidates:
             out.append((self.node_sequences[int(col['ns_idx'][k])], groups, list(zip(dp, tp)), int(col['batches'][k]),
                         part, int(col['num_repartition'][k]), float(cost[k])))
         return out
+
+
+def plan_geometry(space: flatten.FlatPlanSpace, ordinals: np.ndarray) -> Dict[str, np.ndarray]:
+    """row (dg_idx), batches, ns_idx, num_stage and the byte offset of the device-group row of the plans
+    ``ordinals`` of ``space``."""
+    blocks = space.blocks
+    ordinal = np.asarray(ordinals).astype(np.int64)
+    blk = (np.searchsorted(blocks['first_ordinal'], ordinal, side='right') - 1) if len(ordinal) \
+        else np.zeros(0, dtype=np.int64)
+    rel = ordinal - blocks['first_ordinal'][blk]
+    ndiv = len(space.batches)
+    row, stages = rel // ndiv, blocks['num_stage'][blk].astype(np.int64)
+    return dict(row=row, batches=space.batches[rel % ndiv].astype(np.int64),
+                ns_idx=blocks['ns_idx'][blk].astype(np.int64), num_stage=stages,
+                row_byte=blocks['rows_offset'][blk].astype(np.int64) + row * stages)
+
+
+def trace_decoded(lib, p_struct, s_struct, workspace: torch.Tensor, device, ordinals: np.ndarray,
+                  max_stage: int) -> List[list]:
+    """metis_het_trace of ``ordinals`` on the bound problem / space, each plan decoded (verbose.decode_plan).  A plan
+    whose events overflow its buffer is traced again with four times the room."""
+    from . import verbose
+    ordinals = np.ascontiguousarray(ordinals, dtype=np.uint32)
+    out: List[Optional[list]] = [None] * len(ordinals)
+    todo = np.arange(len(ordinals))
+    words = max(256, 64 * (4 * max_stage + 24))
+    while len(todo):
+        n = len(todo)
+        with torch.cuda.device(device):
+            d_ord = torch.from_numpy(ordinals[todo].view(np.int32).copy()).to(device)
+            buf = torch.zeros((max(n, 1), words), dtype=torch.int64, device=device)
+            s = torch.cuda.current_stream(device)
+            rc = lib.metis_het_trace(C.byref(p_struct), C.byref(s_struct), C.c_void_p(d_ord.data_ptr()), C.c_int64(n),
+                                     C.c_void_p(buf.data_ptr()), C.c_int32(words), C.c_void_p(workspace.data_ptr()),
+                                     C.c_int64(workspace.numel()), C.c_void_p(s.cuda_stream))
+            native.check(rc, 'metis_het_trace')
+            host = buf[:n].cpu().numpy().view(np.uint64)
+        again = []
+        for k, i in enumerate(todo.tolist()):
+            if int(host[k, 0]) & 0xFF == verbose.TAG_OVERFLOW:
+                again.append(i)
+            else:
+                out[i] = verbose.decode_plan(host[k])
+        todo = np.asarray(again, dtype=np.int64)
+        words *= 4
+    return out
 
 
 TERM_NAMES = ('execution', 'fb_sync', 'parameter_update', 'dp', 'pp', 'batch_generate')
@@ -620,6 +745,8 @@ class WindowedOutput:
     firsts: np.ndarray                                    # int64, one more than windows searched
     headroom: Optional[np.ndarray] = None                 # float64 aligned with records, when the windows had it
     headroom_s: float = 0.0
+    misses: Optional[np.ndarray] = None                   # MISS_HOST_DTYPE, global ordinals, reference order
+    misses_s: float = 0.0
 
 
 class WindowMerge:
@@ -627,9 +754,13 @@ class WindowMerge:
     step), the fatal ordinal made global.  ``add`` returns True at the first window that reports a fatal plan: the
     reference dies at that plan (quirk Q8), so later windows are not searched."""
 
-    def __init__(self, num_windows: int, with_headroom: bool = False):
-        """``with_headroom``: the windows carry headroom, so an empty result gets an empty headroom array."""
+    def __init__(self, num_windows: int, with_headroom: bool = False, with_misses: bool = False):
+        """``with_headroom``: the windows carry headroom, so an empty result gets an empty headroom array;
+        ``with_misses``: the windows carry their out-of-memory attempts."""
         self.with_headroom = with_headroom
+        self.with_misses = with_misses
+        self._misses: List[np.ndarray] = []
+        self.misses_s = 0.0
         self.summary: Dict[str, object] = {k: 0 for k in _SUMMED_KEYS}
         self.summary.update(fatal_ordinal=_NO_FATAL, fatal_code=0, fatal_aux=0, num_windows=num_windows,
                             windows_searched=0, instantiation=[])
@@ -641,10 +772,22 @@ class WindowMerge:
         self.firsts: List[int] = [0]
 
     def add(self, base: int, summary: Dict[str, int], best, records: Optional[np.ndarray],
-            headroom: Optional[np.ndarray] = None) -> bool:
-        """``headroom``: the window's per-record headroom, aligned with ``records`` (give it for every window or none)."""
+            headroom: Optional[np.ndarray] = None, misses: Optional[np.ndarray] = None) -> bool:
+        """``headroom``: the window's per-record headroom, aligned with ``records`` (give it for every window or none);
+        ``misses``: the window's out-of-memory attempts with window-relative ordinals (native.MISS_DTYPE or
+        MISS_HOST_DTYPE), in (ordinal, call, attempt) order."""
         for k in _SUMMED_KEYS:
             self.summary[k] += int(summary.get(k, 0))
+        if misses is not None:
+            self.summary['num_oom_attempts'] = self.summary.get('num_oom_attempts', 0) + int(
+                summary.get('num_oom_attempts', len(misses)))
+            if len(misses):
+                if misses.dtype == MISS_HOST_DTYPE:
+                    misses = misses.copy()
+                    misses['ordinal'] += int(base)
+                else:
+                    misses = misses_to_host(misses, base)
+                self._misses.append(misses)
         self.summary['windows_searched'] += 1
         if 'instantiation' in summary:
             self.summary['instantiation'].append(summary['instantiation'])
@@ -671,8 +814,12 @@ class WindowMerge:
         if self._headroom or (self.with_headroom and not self._records):
             head = np.concatenate(self._headroom) if self._headroom else np.zeros(0)
             assert len(head) == len(rec), 'headroom given for some windows only'
+        miss = None
+        if self.with_misses or self._misses:
+            miss = np.concatenate(self._misses) if self._misses else np.zeros(0, dtype=MISS_HOST_DTYPE)
+            self.summary.setdefault('num_oom_attempts', len(miss))
         return WindowedOutput(dict(self.summary), self.best, rec, np.asarray(self.bases, dtype=np.int64),
-                              np.asarray(self.firsts, dtype=np.int64), head, self.headroom_s)
+                              np.asarray(self.firsts, dtype=np.int64), head, self.headroom_s, miss, self.misses_s)
 
 
 def window_cost_model(problem: flatten.FlatProblem, lib=None) -> Tuple[float, float, float, float]:
@@ -710,16 +857,17 @@ def agree_budget(budget: float, device) -> float:
 
 
 def search_windows(problem: flatten.FlatProblem, windows: Sequence[flatten.PlanWindow], device=None, rank: int = 0,
-                   world: int = 1, tile: int = 128, headroom: bool = False
+                   world: int = 1, tile: int = 128, headroom: bool = False, misses: bool = False
                    ) -> Tuple[WindowedOutput, DeviceProblem, 'HetSearcher']:
     """Search the windows in ordinal order in ONE DeviceProblem arena (sized for every window up front) with ONE
     HetSearcher (the shard's tiles of every window, workspace sized for the window with the most plans), records only,
     and merge on the host (WindowMerge).  Afterwards the searcher keeps only what rebuilding candidates needs
     (metis_het_detail's workspace): the work lists and the record buffer are released."""
     dp = DeviceProblem(problem, windows[0].space, device, reserve=windows)
-    searcher = HetSearcher(dp, rank, world, tile, want_records=True, want_detail=False, want_headroom=headroom)
+    searcher = HetSearcher(dp, rank, world, tile, want_records=True, want_detail=False, want_headroom=headroom,
+                           want_misses=misses)
     searcher.reserve_workspace(max(w.space.num_plans for w in windows))
-    merge = WindowMerge(len(windows), with_headroom=headroom)
+    merge = WindowMerge(len(windows), with_headroom=headroom, with_misses=misses)
     for w in windows:
         if dp.space is not w.space:                           # the first window was uploaded by the constructor
             dp.reload(problem, w.space)
@@ -727,10 +875,12 @@ def search_windows(problem: flatten.FlatProblem, windows: Sequence[flatten.PlanW
             searcher.rebind()
         out = searcher.run()
         merge.headroom_s += out.headroom_s
+        merge.misses_s += out.misses_s
         if merge.add(w.base, out.summary, out.best, np.array(out.records) if out.records is not None else None,
-                     np.array(out.headroom) if out.headroom is not None else None):
+                     np.array(out.headroom) if out.headroom is not None else None, out.misses):
             break
-    searcher.records = searcher.workspace = searcher.headroom = None
+    searcher.records = searcher.workspace = searcher.headroom = searcher.misses = None
+    searcher.miss_capacity = 0
     searcher.capacity = 0
     with torch.cuda.device(dp.device):
         searcher.workspace = torch.empty(dp.workspace_bytes(0), dtype=torch.uint8, device=dp.device)
@@ -758,6 +908,7 @@ def gather_window_records(merged: WindowedOutput, device) -> WindowedOutput:
     Every rank must have searched the same windows (no fatal plan: api.cost_het_cluster raises before gathering)."""
     import torch.distributed as dist
     world = dist.get_world_size()
+    miss = gather_misses(merged.misses, device) if merged.misses is not None else None   # global ordinals already
     counts = torch.tensor(np.diff(merged.firsts), dtype=torch.int64, device=device)
     all_counts = _gather_rows(counts).numpy().astype(np.int64)     # [world, windows]
     cap = max(int(all_counts.sum(axis=1).max()), 1)
@@ -770,7 +921,8 @@ def gather_window_records(merged: WindowedOutput, device) -> WindowedOutput:
     flat = got.cpu().numpy().view(native.RECORD_DTYPE).reshape(world, cap)
     if merged.headroom is None:
         rec, firsts = merge_rank_windows(all_counts, [flat[r] for r in range(world)])
-        return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts)
+        return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts, misses=miss,
+                              misses_s=merged.misses_s)
     # the headroom travels padded like the records, and is merged with them as one more field of each record
     mine_h = torch.zeros(cap, dtype=torch.float64, device=device)
     if n_local:
@@ -787,7 +939,7 @@ def gather_window_records(merged: WindowedOutput, device) -> WindowedOutput:
     for f, _ in native.RECORD_DTYPE:
         rec[f] = merged_both[f]
     return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts,
-                          np.ascontiguousarray(merged_both['headroom']), merged.headroom_s)
+                          np.ascontiguousarray(merged_both['headroom']), merged.headroom_s, miss, merged.misses_s)
 
 
 def make_window_ranker(searcher: 'HetSearcher', records: np.ndarray, summary: Dict):
@@ -824,8 +976,9 @@ class WindowedCandidates:
 
     def __init__(self, records: np.ndarray, bases: np.ndarray, firsts: np.ndarray,
                  windows: Sequence[flatten.PlanWindow], problem: flatten.FlatProblem, node_sequences: Sequence[Tuple],
-                 searcher: 'HetSearcher', headroom: Optional[np.ndarray] = None):
+                 searcher: 'HetSearcher', headroom: Optional[np.ndarray] = None, misses: Optional[np.ndarray] = None):
         self.records = records
+        self.misses = misses                  # MISS_HOST_DTYPE, global ordinals, reference order; else None
         self.headroom = headroom              # float64 per record (a search with headroom), else None
         self.device = searcher.dp.device      # where the search ran
         self.cost = records['cost']
@@ -871,6 +1024,46 @@ class WindowedCandidates:
             cand = Candidates(rec, detail, dp.space, self.node_sequences, rows_dev=dp.rows_device())
             cand._BULK = 1 << 62                              # gather the rows needed, never the whole blob
             for k, t in zip(at.tolist(), cand.tuples(np.arange(len(rec)))):
+                out[k] = t
+        return out
+
+    def _by_window(self, ordinals: np.ndarray):
+        """(window, positions into ``ordinals``, window-relative ordinals) for every window holding some of them."""
+        ordinals = np.asarray(ordinals, dtype=np.int64)
+        starts = np.asarray([w.base for w in self.windows], dtype=np.int64)
+        win = np.searchsorted(starts, ordinals, side='right') - 1
+        for w in np.unique(win).tolist():
+            at = np.nonzero(win == w)[0]
+            yield w, at, ordinals[at] - starts[w]
+
+    def plan_columns(self, ordinals: np.ndarray) -> Dict[str, np.ndarray]:
+        """Candidates.plan_columns of GLOBAL ordinals, window by window."""
+        n = len(ordinals)
+        out: Dict[str, np.ndarray] = {}
+        for w, at, rel in self._by_window(ordinals):
+            dp = self._load(w)
+            cand = Candidates(np.zeros(0, dtype=native.RECORD_DTYPE), None, dp.space, self.node_sequences,
+                              rows_dev=dp.rows_device())
+            cand._BULK = 1 << 62
+            col = cand.plan_columns(rel)
+            for k, v in col.items():
+                if k not in out:
+                    shape = (n,) + v.shape[1:] if k != 'codes' else (n, native.METIS_MAX_STAGES)
+                    out[k] = np.zeros(shape, dtype=v.dtype)
+                if k == 'codes':
+                    out[k][at, :v.shape[1]] = v
+                else:
+                    out[k][at] = v
+        return out
+
+    def trace(self, ordinals: np.ndarray) -> List[list]:
+        """verbose.decode_plan of GLOBAL ordinals, window by window."""
+        out: List[Optional[list]] = [None] * len(ordinals)
+        for w, at, rel in self._by_window(ordinals):
+            dp = self._load(w)
+            got = trace_decoded(dp.lib, dp.p_struct, dp.s_struct, self.searcher.workspace, dp.device, rel,
+                                int(dp.space.blocks['num_stage'].max()))
+            for k, t in zip(at.tolist(), got):
                 out[k] = t
         return out
 
@@ -1059,8 +1252,9 @@ class HeadroomIndex:
 
 def gather_records(out: HetSearchOutput, searcher: HetSearcher, want_rank: bool = True,
                    counts: Optional[List[int]] = None) -> HetSearchOutput:
-    """Every rank receives every rank's records (+ detail rows): padded tensor all_gathers over NCCL (no pickling),
-    then the merged list is put into estimate_costs order and ranked by the device sort."""
+    """Every rank receives every rank's records (+ detail rows, headroom and misses when the search had them): padded
+    tensor all_gathers over NCCL (no pickling), then the merged list is put into estimate_costs order and ranked by the
+    device sort; the misses are merged into the reference's order (gather_misses)."""
     import torch.distributed as dist
     dev = searcher.dp.device
     world = dist.get_world_size()
@@ -1109,8 +1303,167 @@ def gather_records(out: HetSearchOutput, searcher: HetSearcher, want_rank: bool 
         if head_all is not None:
             headroom_dev = head_all.index_select(0, perm.long())
             headroom = searcher._to_host('headroom_all', headroom_dev, s).view(np.float64)
+    misses = gather_misses(out.misses, dev) if out.misses is not None else None
     return HetSearchOutput(out.summary, out.best, records, detail, out.d2h_bytes, rank_order, detail_dev,
-                           rec_all[:2 * n], headroom, headroom_dev, out.headroom_s)
+                           rec_all[:2 * n], headroom, headroom_dev, out.headroom_s, misses, out.misses_s)
+
+
+# ---------------------------------------------------------------------------------------------
+# out-of-memory partition attempts of a search (misses)
+# ---------------------------------------------------------------------------------------------
+class Misses:
+    """The out-of-memory partition attempts of a search, columnar, in the reference's order (ordinal, call, attempt):
+    every pass of LayerLoadBalancer.partition_layer's loop whose memory test failed (model/load_balancer.py:57-63,
+    127-143).  ``ordinal`` is the inter-stage plan's global ordinal, ``call`` the 0-based partition_layer call of that
+    plan (one per valid strategy it tried), ``attempt`` 1..3, ``deficit`` = -min(memory_state) in MB (> 0) and
+    ``stage`` the lowest stage with that smallest state."""
+
+    def __init__(self, table: np.ndarray):
+        self.table = table                                    # MISS_HOST_DTYPE
+        self.ordinal = table['ordinal'].astype(np.int64)
+        self.call = table['call'].astype(np.int64)
+        self.attempt = table['attempt'].astype(np.int64)
+        self.stage = table['stage'].astype(np.int64)
+        self.num_stage = table['num_stage'].astype(np.int64)
+        self.deficit = np.ascontiguousarray(table['deficit'])
+
+    def __len__(self) -> int:
+        return len(self.table)
+
+
+def closest_order(deficit: np.ndarray, device=None) -> np.ndarray:
+    """Positions of the misses by ascending deficit, ties in reference order: metis_sort_records(METIS_SORT_RANKED) on
+    MetisMiss rows whose ordinal field holds the position (the rows are already in reference order)."""
+    n = len(deficit)
+    if n == 0:
+        return np.zeros(0, dtype=np.int64)
+    if n > 0xFFFFFFFF:
+        raise NotImplementedError(f'ordering {n} misses: positions are 32-bit')
+    dev = _require_cuda(device)
+    lib = native.load_library()
+    rows = np.zeros(n, dtype=native.MISS_DTYPE)
+    rows['deficit'] = deficit
+    rows['ordinal'] = np.arange(n, dtype=np.uint32)
+    with torch.cuda.device(dev):
+        buf = torch.from_numpy(rows.view(np.int64).copy()).to(dev)
+        ws = torch.empty(int(lib.metis_sort_workspace_bytes(C.c_int64(n))), dtype=torch.uint8, device=dev)
+        perm = torch.empty(n, dtype=torch.int32, device=dev)
+        s = torch.cuda.current_stream(dev)
+        rc = lib.metis_sort_records(C.c_void_p(buf.data_ptr()), C.c_int64(n), C.c_int32(native.SORT_RANKED),
+                                    C.c_void_p(perm.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_int64(ws.numel()),
+                                    C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_sort_records')
+        return perm.cpu().numpy().view(np.uint32).astype(np.int64)
+
+
+def _find_attempt(items: list, call: int, attempt: int):
+    """The TraceCall of partition_layer call ``call`` and its TraceAttempt ``attempt`` in a decoded plan."""
+    from .verbose import TraceCall
+    calls = [it for it in items if isinstance(it, TraceCall)]
+    c = calls[call]
+    for a in c.attempts:
+        if a.attempt == attempt:
+            return c, a
+    raise AssertionError(f'attempt {attempt} of call {call} not in the replay')
+
+
+def replay_misses(candidates, misses: Misses, idx: np.ndarray):
+    """(plan columns, [(TraceCall, TraceAttempt)]) of the misses ``idx``: each distinct plan is replayed once by
+    metis_het_trace, and the failed attempt is looked up in its decoded events."""
+    idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+    ords = misses.ordinal[idx]
+    uniq, inv = np.unique(ords, return_inverse=True)
+    traced = candidates.trace(uniq) if len(uniq) else []
+    found = [_find_attempt(traced[inv[k]], int(misses.call[i]), int(misses.attempt[i])) for k, i in enumerate(idx)]
+    return candidates.plan_columns(ords), found
+
+
+def miss_tuples(candidates, misses: Misses, idx) -> List[Tuple]:
+    """(node_sequence, device_groups, strategies, batches, layer_partition, attempt, deficit, stage) of misses ``idx``."""
+    idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+    if not len(idx):
+        return []
+    col, found = replay_misses(candidates, misses, idx)
+    out = []
+    for k, i in enumerate(idx.tolist()):
+        S = int(col['num_stage'][k])
+        groups = (1 << col['codes'][k, :S].astype(np.int64)).tolist()
+        call, att = found[k]
+        strategies = [(g >> t, 1 << t) for g, t in zip(groups, call.tpc)]
+        out.append((candidates.node_sequences[int(col['ns_idx'][k])], groups, strategies, int(col['batches'][k]),
+                    list(att.partition), int(misses.attempt[i]), float(misses.deficit[i]), int(misses.stage[i])))
+    return out
+
+
+@dataclass
+class MissDetail:
+    """Per-stage values of chosen misses, one row per miss in the order asked for; NaN past a miss's stages."""
+    performance: np.ndarray       # [n, width]: stage performance fed to the attempt's balancer run
+    memory_capacity: np.ndarray   # stage_memory_capacity
+    memory_demand: np.ndarray     # stage_memory_demand of the attempt
+    memory_state: np.ndarray      # memory_state (capacity - demand) of the attempt
+    num_stage: np.ndarray
+
+    def __len__(self) -> int:
+        return len(self.num_stage)
+
+
+def memory_capacity(problem: flatten.FlatProblem, ns_idx: int, groups: Sequence[int]) -> List[float]:
+    """StagePerformance.get_device_group_memory_capacity of every stage (model/device_group.py:87-101), like
+    PlanEvaluator::memory_capacity: the stage's devices of each type run, summed in run order."""
+    a = problem.arrays
+    mem, typ, end = a['type_memory'], a['ns_run_type'][ns_idx], a['ns_run_end'][ns_idx]
+    out, lo_rank = [], 0
+    for g in groups:
+        hi_rank = lo_rank + g
+        if len(mem) == 1:
+            out.append(float(mem[0]) * float(g))
+        else:
+            terms, lo = [], 0
+            for k in range(len(end)):
+                hi = int(end[k])
+                x, y = max(lo_rank, lo), min(hi_rank, hi)
+                if y > x:
+                    terms.append(float(mem[typ[k]]) * float(y - x))
+                lo = hi
+            out.append(sum(terms))
+        lo_rank = hi_rank
+    return out
+
+
+def miss_detail(candidates, misses: Misses, idx) -> MissDetail:
+    idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+    width = max(int(misses.num_stage[idx].max()), 1) if len(idx) else 1
+    f = {k: np.full((len(idx), width), np.nan) for k in ('performance', 'memory_capacity', 'memory_demand',
+                                                          'memory_state')}
+    if len(idx):
+        col, found = replay_misses(candidates, misses, idx)
+        for k in range(len(idx)):
+            S = int(col['num_stage'][k])
+            groups = (1 << col['codes'][k, :S].astype(np.int64)).tolist()
+            _call, att = found[k]
+            f['performance'][k, :S] = att.performance
+            f['memory_capacity'][k, :S] = memory_capacity(candidates.problem, int(col['ns_idx'][k]), groups)
+            f['memory_demand'][k, :S] = att.demand
+            f['memory_state'][k, :S] = att.state
+    return MissDetail(num_stage=misses.num_stage[idx].copy(), **f)
+
+
+def gather_misses(misses: np.ndarray, device) -> np.ndarray:
+    """Multi-rank: every rank receives every rank's misses (MISS_HOST_DTYPE, global ordinals), padded like the records
+    (one all_gather of the counts, one of the rows), merged into the reference's order."""
+    import torch.distributed as dist
+    world = dist.get_world_size()
+    counts = _gather_rows(torch.tensor([len(misses)], dtype=torch.int64, device=device)).numpy().reshape(-1)
+    cap = max(int(counts.max()), 1)
+    words = MISS_HOST_DTYPE.itemsize // 8
+    mine = torch.zeros(cap * words, dtype=torch.int64, device=device)
+    if len(misses):
+        mine[:len(misses) * words] = torch.from_numpy(np.ascontiguousarray(misses).view(np.int64).reshape(-1)).to(device)
+    got = torch.empty(world * cap * words, dtype=torch.int64, device=device)
+    dist.all_gather_into_tensor(got, mine)
+    flat = got.cpu().numpy().view(MISS_HOST_DTYPE).reshape(world, cap)
+    return position_order(np.concatenate([flat[r, :int(counts[r])] for r in range(world)]))
 
 
 # ---------------------------------------------------------------------------------------------

@@ -14,6 +14,7 @@ from __future__ import annotations
 
 import ctypes as C
 from collections import Counter
+from dataclasses import dataclass, field
 from typing import Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -111,11 +112,106 @@ def trace_plans(dp, ordinals: np.ndarray, words_per_plan: int = 0) -> np.ndarray
         return trace[:n].cpu().numpy().view(np.uint64)
 
 
-def format_plan(words: np.ndarray, plan, gpu_cluster, max_tp: int, max_bs: int) -> Iterator[str]:
-    """Lines of one inter-stage plan (the body of the loop at cost_het_cluster.py:31-48)."""
+@dataclass
+class TraceAttempt:
+    """One partition attempt of a partition_layer call (model/load_balancer.py:127-143)."""
+    attempt: int                  # 1..3
+    performance: List[float]      # stage performance fed to this attempt's balancer run
+    partition: List[int]          # layer_partition
+    demand: List[float]           # stage_memory_demand
+    state: List[float]            # memory_state
+
+
+@dataclass
+class TraceCall:
+    """One partition_layer call: the valid strategy it was made for and what it printed, in order."""
+    tpc: List[int]                # log2(tp) per stage
+    performance: Optional[List[float]] = None             # stage_compute_performance (None: fatal before it)
+    events: list = field(default_factory=list)            # ('attempt', TraceAttempt) / ('adjust', aux, values or None)
+    accepted: int = 0             # attempt number accepted, 0 = layer_partition None
+    fatal: Optional[Tuple[int, int]] = None               # (code, aux): the reference aborts inside this call
+
+    @property
+    def attempts(self) -> List[TraceAttempt]:
+        return [e[1] for e in self.events if e[0] == 'attempt']
+
+
+@dataclass
+class TraceCost:
+    """The costing of an accepted call: the data loadbalancer splits, then a KeyError or the cost terms."""
+    splits: List[List[int]]
+    keyerror: Optional[Tuple[int, int, int]] = None       # (site, a, b)
+    terms: Optional[List[float]] = None                   # execution, fb_sync, update, dp, pp, cost
+
+
+def decode_plan(words: np.ndarray) -> list:
+    """One plan's event stream (metis_trace.cuh) -> its items in order: TraceCall, a TraceCost after every accepted
+    call, and ('fatal', code, aux) when the reference aborts before a call's strategy is recorded."""
     ev = _Events(words)
     if ev.peek() == TAG_OVERFLOW:
         raise native.MetisNativeError('trace buffer too small for this plan; raise words_per_plan')
+    items: list = []
+    while True:
+        tag, n, aux = ev.head()
+        if tag == TAG_END:
+            return items
+        if tag == TAG_FATAL:
+            items.append(('fatal', aux, ev.ints(1)[0]))
+            return items
+        assert tag == TAG_STRATEGY, tag
+        call = TraceCall(ev.packed(n, 8))
+        items.append(call)
+        tag, n, aux = ev.head()
+        if tag == TAG_FATAL:
+            call.fatal = (aux, ev.ints(1)[0])
+            return items
+        assert tag == TAG_PERF
+        call.performance = perf = ev.floats(n)
+        while True:                                           # partition_layer, load_balancer.py:127-144
+            tag, n, aux = ev.head()
+            if tag == TAG_FATAL:
+                call.fatal = (aux, ev.ints(1)[0])
+                return items
+            if tag == TAG_RESULT:
+                call.accepted = aux
+                break
+            if tag == TAG_ATTEMPT:
+                part = ev.packed(n + 1, 16)
+                demand, state = ev.floats(n), ev.floats(n)
+                call.events.append(('attempt', TraceAttempt(aux, perf, part, demand, state)))
+            elif tag == TAG_ADJUST:
+                values = ev.floats(n) if n else None
+                call.events.append(('adjust', aux, values))
+                if values is not None:
+                    perf = values
+            else:
+                raise AssertionError(f'unexpected trace tag {tag}')
+        if not call.accepted:
+            continue
+        cost = TraceCost([])
+        items.append(cost)
+        while True:
+            tag, n, aux = ev.head()
+            if tag == TAG_SPLIT:
+                cost.splits.append(ev.ints(n))
+            elif tag == TAG_KEYERROR:
+                a, b = ev.ints(2)
+                cost.keyerror = (aux, a, b)
+                break
+            elif tag == TAG_COST:
+                cost.terms = ev.floats(6)
+                break
+            else:
+                raise AssertionError(f'unexpected trace tag {tag}')
+
+
+def _fatal(code: int, aux: int):
+    return native.MetisNativeError(f'the reference aborts at this plan (fatal code {code}, aux {aux})')
+
+
+def format_plan(words: np.ndarray, plan, gpu_cluster, max_tp: int, max_bs: int) -> Iterator[str]:
+    """Lines of one inter-stage plan (the body of the loop at cost_het_cluster.py:31-48)."""
+    items = iter(decode_plan(words))
     yield ''
     yield ''
     yield f'inter_stage_plan: {plan}'
@@ -155,41 +251,29 @@ def format_plan(words: np.ndarray, plan, gpu_cluster, max_tp: int, max_bs: int) 
             if bad:
                 yield bad
                 continue
-            tag, n, _ = ev.head()
-            if tag == TAG_FATAL:
-                raise native.MetisNativeError(f'the reference aborts at this plan (fatal code {_}, aux {ev.ints(1)[0]})')
-            assert tag == TAG_STRATEGY and n == len(groups), (tag, n)
-            tpc = ev.packed(n, 8)
-            assert [(g >> t, 1 << t) for g, t in zip(groups, tpc)] == strategies, 'device and host disagree on the chain'
+            call = next(items)
+            if isinstance(call, tuple):
+                raise _fatal(call[1], call[2])
+            assert isinstance(call, TraceCall) and len(call.tpc) == len(groups), call
+            assert [(g >> t, 1 << t) for g, t in zip(groups, call.tpc)] == strategies, 'device and host disagree on the chain'
             yield f'valid_strategies: {strategies}'
-            tag, n, aux = ev.head()
-            if tag == TAG_FATAL:
-                raise native.MetisNativeError(f'the reference aborts at this plan (fatal code {aux}, aux {ev.ints(1)[0]})')
-            assert tag == TAG_PERF
-            perf = ev.floats(n)
+            if call.performance is None:
+                raise _fatal(*call.fatal)
             yield f'stage_memory_capacity: {_memory_capacity(gpu_cluster, rank_types, groups)}'
-            yield f'stage_compute_performance: {perf}'
-            while True:                                       # partition_layer, load_balancer.py:127-144
-                tag, n, aux = ev.head()
-                if tag == TAG_FATAL:
-                    raise native.MetisNativeError(f'the reference aborts at this plan (fatal code {aux}, aux {ev.ints(1)[0]})')
-                if tag == TAG_RESULT:
-                    break
-                if tag == TAG_ATTEMPT:
-                    part = ev.packed(n + 1, 16)
-                    demand, state = ev.floats(n), ev.floats(n)
-                    yield f'layer_partition: {part}'
-                    yield f'stage_memory_demand: {demand}, memory_state: {state}'
-                    last_part, last_state = part, state
-                elif tag == TAG_ADJUST:
-                    if n == 0:
-                        yield 'Even with the reallocation of layers, memory issues persist.'
-                    else:
-                        yield f'adj_stage_compute_performance({aux}): {ev.floats(n)}'
+            yield f'stage_compute_performance: {call.performance}'
+            for e in call.events:
+                if e[0] == 'attempt':
+                    yield f'layer_partition: {e[1].partition}'
+                    yield f'stage_memory_demand: {e[1].demand}, memory_state: {e[1].state}'
+                    last_part, last_state = e[1].partition, e[1].state
+                elif e[2] is None:
+                    yield 'Even with the reallocation of layers, memory issues persist.'
                 else:
-                    raise AssertionError(f'unexpected trace tag {tag}')
-            if aux:                                           # success at attempt `aux`
-                partition, memory_state, nrep = last_part, last_state, aux
+                    yield f'adj_stage_compute_performance({e[1]}): {e[2]}'
+            if call.fatal is not None:
+                raise _fatal(*call.fatal)
+            if call.accepted:                                 # success at attempt `accepted`
+                partition, memory_state, nrep = last_part, last_state, call.accepted
                 yield f'layer_partition: {partition}'
                 break
             memory_state = None
@@ -197,22 +281,16 @@ def format_plan(words: np.ndarray, plan, gpu_cluster, max_tp: int, max_bs: int) 
         # cost_het_cluster.py:38-48
         yield (f'node_sequence: {plan.node_sequence}, device_group: {plan.device_groups}, num_stage: {plan.num_stage}, '
                f'batches: {plan.batches}, gbs: {plan.gbs}, strategies: {strategies}, layer_partition: {partition}')
-        while True:
-            tag, n, aux = ev.head()
-            if tag == TAG_SPLIT:
-                yield f'data loadbalancer: {ev.ints(n)}'
-            elif tag == TAG_KEYERROR:
-                a, b = ev.ints(2)
-                yield f'KeyError: {_key_error_text(aux, a, b)}'
-                break
-            elif tag == TAG_COST:
-                c = ev.floats(6)
-                yield (f'execution_cost: {c[0]}, fb_sync_cost: {c[1]}, parameter_upate_costs: {c[2]}, dp_cost: {c[3]}, '
-                       f'pp_cost: {c[4]}')
-                yield f'cost: {c[5]}'
-                break
-            else:
-                raise AssertionError(f'unexpected trace tag {tag}')
+        cost = next(items)
+        for split in cost.splits:
+            yield f'data loadbalancer: {split}'
+        if cost.keyerror is not None:
+            yield f'KeyError: {_key_error_text(*cost.keyerror)}'
+        else:
+            c = cost.terms
+            yield (f'execution_cost: {c[0]}, fb_sync_cost: {c[1]}, parameter_upate_costs: {c[2]}, dp_cost: {c[3]}, '
+                   f'pp_cost: {c[4]}')
+            yield f'cost: {c[5]}'
 
 
 def plan_transcript(args, gpu_cluster, profile_data, model_config, layer_load_balancer=None,
