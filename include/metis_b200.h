@@ -304,6 +304,36 @@ int metis_het_breakdown(const MetisProblem *problem, const MetisPlanSpace *space
                         int64_t workspace_bytes, void *stream);
 
 /*
+ * Network what-if: HeteroCostEstimator.get_cost (model/cost_estimator.py:199-244) of costed candidates under other
+ * bandwidth tables.  Bandwidth enters only the cost model, so the strategies and partition a search found stay valid;
+ * each candidate is re-costed from its detail row with no balancer run.  Every scenario goes through the general
+ * (non-uniform) bandwidth path; under the search's own tables the costs equal the search's bit for bit.
+ *   records    [device] n MetisRecord of one search (any order); only ordinal is read
+ *   detail     [device] n rows of detail_stride bytes: dp codes[S], tp codes[S], partition[S+1], as the search writes
+ *              them; detail_stride >= 3 * space->max_stage + 1
+ *   bandwidths [device] num_scenarios x 2 x num_types doubles: bw_first[T] then bw_min[T] of each scenario
+ *              (MetisProblem.type_bw_first / type_bw_min)
+ *   costs      [device] num_scenarios x n doubles: costs[j * n + i] is record i's cost under scenario j; NaN when its
+ *              replay raises a KeyError (cannot happen for a record the search costed)
+ *   workspace  [device] metis_het_workspace_bytes(problem, 0, 1) bytes
+ */
+int metis_het_recost(const MetisProblem *problem, const MetisPlanSpace *space, const MetisRecord *records, int64_t n,
+                     const uint8_t *detail, int32_t detail_stride, const double *bandwidths, int32_t num_scenarios,
+                     double *costs, void *workspace, int64_t workspace_bytes, void *stream);
+
+/*
+ * Regret of re-costed candidates: best[j] = min_i costs[j * n + i] and regret[i] = max_j (costs[j * n + i] - best[j]),
+ * in fp64 (absolute, not a ratio: costs of rough profiles may be negative).  Exact, whatever the reduction order.
+ * NaN costs are skipped by the min.  With n == 0, best[j] = +inf.
+ *   costs     [device] num_scenarios x n doubles (metis_het_recost's layout), 1 <= num_scenarios <= 65535
+ *   best      [device] num_scenarios doubles;  regret [device] n doubles
+ *   workspace [device] metis_recost_regret_workspace_bytes(num_scenarios, n) bytes
+ */
+int64_t metis_recost_regret_workspace_bytes(int32_t num_scenarios, int64_t n);
+int metis_recost_regret(const double *costs, int32_t num_scenarios, int64_t n, double *best, double *regret,
+                        void *workspace, int64_t workspace_bytes, void *stream);
+
+/*
  * metis_homo_cost with the cost terms and the per-stage memory sums (HomoCostEstimator.get_cost returns them as
  * stage_memory, model/cost_estimator.py:121-138).
  *   terms        [device] n x 6 doubles: execution, fb_sync, parameter update, dp, pp, batch generate

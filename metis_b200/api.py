@@ -19,6 +19,7 @@ holders of inputs - every evaluation happens on the GPU (metis_b200.search).
 from __future__ import annotations
 
 import argparse
+import math
 import time
 from dataclasses import dataclass
 from itertools import permutations
@@ -184,6 +185,7 @@ class HetSearchResult(Sequence):
         self.timings = timings or {}
         self._ranker = ranker                 # () -> uint32 permutation, the stable device sort by cost
         self._best_key = best_key             # (ordinal, step) of the argmin found by the search kernels
+        self._searched = None                 # cluster_signature of the cluster searched (cost_het_cluster sets it)
 
     def __len__(self) -> int:
         return len(self.candidates)
@@ -311,6 +313,30 @@ class HetSearchResult(Sequence):
                 raise IndexError('list index out of range')
         return self.candidates.breakdown(pos, per_stage)
 
+    def recost(self, clusters: Sequence) -> 'search.Recost':
+        """Network what-if: every candidate re-costed under each GPUCluster of ``clusters`` on the GPU
+        (metis_het_recost), with no new search.  Bandwidth enters only the cost model (model/cost_estimator.py:205-232),
+        so a search under a cluster that differs from the searched one only in bandwidth returns the same candidates
+        with these costs, bit for bit.  Each cluster must therefore have the searched hostfile entries (ip and GPU
+        count, in order) and the same instance_type and memory on every node; every bandwidth the model reads
+        (intra_bandwidth, and inter_bandwidth when the search used 'Q2') must be finite and > 0.  The corrections of
+        the search apply to every scenario.  Returns a search.Recost: ``costs`` [K, N], ``ranked(j, k)``, ``best(j)``,
+        ``regret`` and ``robust(k)``.  With torch.distributed every rank holds all candidates: no collective is
+        issued."""
+        from . import search
+        if self._searched is None:
+            raise ValueError('this result does not know the cluster it was searched on: no recost')
+        clusters = list(clusters)
+        if not clusters:
+            raise ValueError('recost needs at least one cluster')
+        corrected = tuple(self.summary.get('corrected', ()))
+        type_names = self.candidates.problem.type_names
+        bw = np.empty((len(clusters), 2, len(type_names)), dtype=np.float64)
+        for j, cluster in enumerate(clusters):
+            check_scenario(self._searched, cluster, type_names, corrected, j)
+            bw[j, 0], bw[j, 1] = flatten.cluster_bandwidths(cluster, type_names, corrected)
+        return self.candidates.recost(bw)
+
     def best(self) -> Optional[Tuple]:
         """argmin (cost, position): the first entry of the ranked list.  The search kernels reduce it on the device
         (het_finalize_kernel: lowest cost, then lowest ordinal, then lowest step), so no sort is needed for it."""
@@ -320,6 +346,46 @@ class HetSearchResult(Sequence):
                 return self.candidates.tuples([at])[0]
         top = self.ranked(1)
         return top[0] if top else None
+
+
+def cluster_signature(gpu_cluster, type_names: Sequence[str]) -> Tuple[list, list]:
+    """What a network what-if must keep from the searched cluster: (ip, GPU count, instance_type, memory) of every
+    hostfile entry in order, and the memory each device type of ``type_names`` is given (the first clusterfile entry of
+    the type, gpu_cluster.py:47-50)."""
+    nodes = []
+    for h in gpu_cluster.host_entries.values():
+        info = gpu_cluster.nodes_info.get(h['ip'], {})
+        nodes.append((h['ip'], h['num_device'], info.get('instance_type'), info.get('memory')))
+    return nodes, [gpu_cluster.get_device_memory_for_device_type(t) for t in type_names]
+
+
+_NODE_FIELDS = ('ip', 'GPU count', 'instance_type', 'memory')
+
+
+def check_scenario(searched: Tuple[list, list], cluster, type_names: Sequence[str], corrected: Sequence[str],
+                   j: int) -> None:
+    """ValueError, naming the node and the field, unless ``cluster`` (scenario j) differs from the searched cluster
+    only in bandwidth and has a finite bandwidth > 0 wherever the cost model reads one."""
+    nodes, type_memory = searched
+    got, got_memory = cluster_signature(cluster, type_names)
+    if len(got) != len(nodes):
+        raise ValueError(f'cluster {j}: {len(got)} hostfile entries, the searched cluster has {len(nodes)}')
+    for k, (want, have) in enumerate(zip(nodes, got)):
+        for field, a, b in zip(_NODE_FIELDS, want, have):
+            if a != b:
+                raise ValueError(f'cluster {j}, node {k} ({have[0]}): {field} is {b!r}, the searched cluster has {a!r}')
+    for name, a, b in zip(type_names, type_memory, got_memory):
+        if a != b:
+            raise ValueError(f'cluster {j}, device type {name}: memory (its first clusterfile entry) is {b!r}, the '
+                             f'searched cluster has {a!r}')
+    fields = ('intra_bandwidth', 'inter_bandwidth') if 'Q2' in corrected else ('intra_bandwidth',)
+    for k, h in enumerate(cluster.host_entries.values()):
+        info = cluster.nodes_info[h['ip']]
+        for field in fields:
+            v = info.get(field)
+            ok = isinstance(v, (int, float)) and not isinstance(v, bool) and math.isfinite(v) and v > 0
+            if not ok:
+                raise ValueError(f'cluster {j}, node {k} ({h["ip"]}): {field} must be a finite number > 0, not {v!r}')
 
 
 def het_problem(args, gpu_cluster, profile_data, model_config, layer_load_balancer=None,
@@ -436,6 +502,7 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
         result = _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1, headroom,
                                    misses)
         result.summary['listing'] = 'host' if listing is None else 'device'
+        result._searched = cluster_signature(gpu_cluster, problem.type_names)
         return result
     stride = 3 * int(space.blocks['num_stage'].max()) + 1
     dp, searcher = _engine(problem, space, dev, rank, world, stride)
@@ -488,6 +555,7 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
                              best_key=(best[1], best[2]) if best else None)
     result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
                       'decode_columns_s': time.perf_counter() - t2}
+    result._searched = cluster_signature(gpu_cluster, problem.type_names)
     if headroom:
         result.timings['headroom_s'] = out.headroom_s
     if misses:

@@ -22,7 +22,7 @@
 
 #if defined(__CUDACC__)
 #define MB_HD __host__ __device__ __forceinline__
-#define MB_HD_NOINLINE __host__ __device__ __noinline__
+#define MB_HD_NOINLINE __host__ __device__ __noinline__ inline   // inline: one definition across translation units
 #else
 #define MB_HD inline
 #define MB_HD_NOINLINE inline

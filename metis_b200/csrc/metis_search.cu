@@ -23,7 +23,8 @@
 //   homo_cost_kernel      a17: one thread per UniformPlan
 //   homo_breakdown_kernel the same with the cost terms and per-stage memory
 //   layer_balance_kernel  a10 alone, for unit parity
-//   (rank_records_kernel, the stable record sort, lives in metis_rank.cu; the headroom select / front in metis_select.cu)
+//   (rank_records_kernel, the stable record sort, lives in metis_rank.cu; the headroom select / front in metis_select.cu;
+//   het_recost_kernel and the regret reductions in metis_recost.cu)
 //   het_first_kernel and het_chain_kernel are compiled per output mask OUT (kOutHeadroom | kOutMisses): the side
 //   outputs of metis_het_search_outputs exist only in the instantiations that write them
 //
@@ -38,6 +39,7 @@
 #include <type_traits>
 
 #include "metis_eval.cuh"
+#include "metis_blob.cuh"
 #include "metis_coop.cuh"
 #include "metis_warp.cuh"
 #include "metis_trace.cuh"
@@ -81,61 +83,6 @@ static int arg_fail(const char *what) {
 }
 int fail_cuda(cudaError_t e, const char *what) { return cuda_fail(e, what); }   // metis_internal.h
 int fail_arg(const char *what) { return arg_fail(what); }
-
-struct BlobLayout {
-    uint32_t total;               // bytes staged into shared memory
-    uint32_t key, lc, mem, exec_full, fb, norm, derived, tmem, bwf, bwm, runt, rune, q10e;
-    uint32_t rsum, rsum_bytes;    // range-sum tables (Tables::rsum): behind the staged part, read from L2
-};
-
-static uint32_t align16(uint32_t v) { return (v + 15u) & ~15u; }
-
-static BlobLayout make_layout(const MetisProblem &p) {
-    BlobLayout l;
-    uint32_t o = 0;
-    const uint32_t nkey = (uint32_t)p.num_types * p.num_tp * p.num_bs;
-    l.key = o;       o = align16(o + nkey * 2);
-    l.lc = o;        o = align16(o + (uint32_t)p.num_keys * p.lpad * 8);
-    l.mem = o;       o = align16(o + (uint32_t)p.num_keys * p.lpad * 8);
-    l.exec_full = o; o = align16(o + (uint32_t)p.num_keys * 8);
-    l.fb = o;        o = align16(o + (uint32_t)p.num_keys * 8);
-    l.norm = o;      o = align16(o + (uint32_t)p.norm_len * 8);
-    l.derived = o;   o = align16(o + (uint32_t)derived_layout(p).total * 8);
-    l.tmem = o;      o = align16(o + (uint32_t)p.num_types * 8);
-    l.bwf = o;       o = align16(o + (uint32_t)p.num_types * 8);
-    l.bwm = o;       o = align16(o + (uint32_t)p.num_types * 8);
-    l.runt = o;      o = align16(o + (uint32_t)p.num_node_sequences * p.num_types);
-    l.rune = o;      o = align16(o + (uint32_t)p.num_node_sequences * p.num_types * 4);
-    l.q10e = o;      o = align16(o + (uint32_t)p.num_node_sequences * p.num_types * 4);
-    l.total = o;
-    const uint64_t n = (uint64_t)p.num_layers + 1;
-    l.rsum = (o + 127u) & ~127u;
-    l.rsum_bytes = (uint32_t)((uint64_t)(2 * p.num_keys + 1) * n * n * 8);    // <= 2 * 255 keys... checked in check_problem
-    return l;
-}
-
-// `base`: the staged tables (shared or global memory); `gblob`: the blob in global memory when its range-sum tables
-// were filled for this launch (search kernels), else nullptr
-__device__ __forceinline__ Tables make_tables(const MetisProblem &p, const BlobLayout &l, const uint8_t *base,
-                                              const uint8_t *gblob = nullptr) {
-    Tables T;
-    T.p = p;
-    T.rsum = gblob ? reinterpret_cast<const double *>(gblob + l.rsum) : nullptr;
-    T.key_index = reinterpret_cast<const int16_t *>(base + l.key);
-    T.lc = reinterpret_cast<const double *>(base + l.lc);
-    T.mem = reinterpret_cast<const double *>(base + l.mem);
-    T.exec_full = reinterpret_cast<const double *>(base + l.exec_full);
-    T.fb_sync = reinterpret_cast<const double *>(base + l.fb);
-    T.norm_lc = reinterpret_cast<const double *>(base + l.norm);
-    bind_derived(T, reinterpret_cast<const double *>(base + l.derived));
-    T.type_memory = reinterpret_cast<const double *>(base + l.tmem);
-    T.bw_first = reinterpret_cast<const double *>(base + l.bwf);
-    T.bw_min = reinterpret_cast<const double *>(base + l.bwm);
-    T.run_type = base + l.runt;
-    T.run_end = reinterpret_cast<const int32_t *>(base + l.rune);
-    T.q10_end = reinterpret_cast<const int32_t *>(base + l.q10e);
-    return T;
-}
 
 __device__ __forceinline__ void copy_bytes(uint8_t *dst, const void *src, uint32_t n, uint32_t tid, uint32_t nthr) {
     const uint8_t *s = static_cast<const uint8_t *>(src);
@@ -222,42 +169,6 @@ __device__ __forceinline__ const Tables &block_tables(Tables &s_tables, const Me
     if (use_smem) stage_blob_tma(smem, blob, lay.total, mbar);     // its __syncthreads publishes s_tables
     else __syncthreads();
     return s_tables;
-}
-
-// ---- ordinal -> plan ---------------------------------------------------------------------------
-__device__ __forceinline__ int find_block(const MetisPlanSpace &sp, int64_t ordinal) {
-    int lo = 0, hi = sp.num_blocks - 1;
-    while (lo < hi) {                                         // last block with first_ordinal <= ordinal
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(&sp.blocks[mid].first_ordinal) <= ordinal) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
-
-// `hint` >= 0: a block known to start at or before `ordinal` (the warp's first plan); blocks are walked
-// forward from it, so the 32 consecutive plans of a warp cost one binary search instead of 32.
-__device__ __forceinline__ bool decode_plan(const MetisPlanSpace &sp, int64_t ordinal, PlanDesc &pd, int hint = -1) {
-    if (ordinal < 0 || ordinal >= sp.num_plans) return false;
-    int lo;
-    if (hint >= 0) {
-        lo = hint;
-        while (lo + 1 < sp.num_blocks && __ldg(&sp.blocks[lo + 1].first_ordinal) <= ordinal) ++lo;
-    } else {
-        lo = find_block(sp, ordinal);
-    }
-    const MetisPlanBlock b = sp.blocks[lo];
-    const int64_t rel = ordinal - b.first_ordinal;
-    const int64_t row = rel / sp.num_div;
-    const int div = (int)(rel - row * sp.num_div);
-    pd.ordinal = (uint32_t)ordinal;
-    pd.ns = b.ns_idx;
-    pd.S = b.num_stage;
-    pd.label = b.label_stage;
-    pd.batches = __ldg(&sp.batches[div]);
-    const int64_t off = b.rows_offset + row * b.num_stage;
-    pd.row = sp.rows + off;
-    pd.geo = pack_geo(off, b.num_stage, b.label_stage, b.ns_idx, div);
-    return true;
 }
 
 // task list entry -> plan (no block search: the geometry word was stored at admission)
@@ -1207,6 +1118,23 @@ int metis_het_detail(const MetisProblem *problem, const MetisPlanSpace *space, c
     if (e != cudaSuccess) return cuda_fail(e, "het_detail_kernel");
     return METIS_OK;
 }
+
+}  // extern "C"
+
+int metis::stage_replay_tables(const MetisProblem *problem, void *workspace, int64_t workspace_bytes, cudaStream_t stream,
+                               BlobLayout &lay, const uint8_t *&blob) {
+    int rc = check_problem(problem);
+    if (rc) return rc;
+    if (!workspace) return arg_fail("NULL argument");
+    lay = make_layout(*problem);
+    if (workspace_bytes < 256 + kFixedWs + (int64_t)align16(lay.total)) return METIS_E_CAPACITY;
+    const Workspace ws = carve(workspace, lay);
+    pack_tables_kernel<<<8, 256, 0, stream>>>(*problem, lay, ws.blob);
+    blob = ws.blob;
+    return METIS_OK;
+}
+
+extern "C" {
 
 int metis_het_trace(const MetisProblem *problem, const MetisPlanSpace *space, const uint32_t *ordinals, int64_t n,
                     uint64_t *trace, int32_t words_per_plan, void *workspace, int64_t workspace_bytes, void *stream_) {

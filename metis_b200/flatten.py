@@ -88,6 +88,26 @@ def norm_layer_duration(profile_data: Dict) -> List[float]:
     return [d / total for d in durations]
 
 
+def cluster_bandwidths(gpu_cluster, type_names: Sequence[str], corrected: Sequence[str] = ()
+                       ) -> Tuple[List[float], List[float]]:
+    """The bandwidth tables the cost model reads, one entry per device type of ``type_names``: bw_first[T] is the
+    intra_bandwidth of the type's first node (cluster_bandwidth.py:49-54), bw_min[T] the smallest between-node
+    bandwidth of its nodes (:56-68), which gpu_cluster.py:56-58 reads from intra_bandwidth (quirk Q2) or, with 'Q2' in
+    ``corrected``, from the clusterfile's inter_bandwidth.  MetisProblem.type_bw_first / type_bw_min and the scenarios
+    of HetSearchResult.recost both come from here."""
+    bw_first, bw_min = [], []
+    node_ids = list(gpu_cluster.nodes.keys())
+    for name in type_names:
+        mine = [i for i in node_ids if _type_name(gpu_cluster.nodes[i].device_type) == name]
+        bw_first.append(float(gpu_cluster.get_intra_bandwidth(mine[0])))
+        if 'Q2' in corrected:
+            bw_min.append(float(min(gpu_cluster.nodes_info[gpu_cluster.host_entries[i]['ip']]['inter_bandwidth']
+                                    for i in mine)))
+        else:
+            bw_min.append(float(min(gpu_cluster.get_inter_bandwidth(i) for i in mine)))
+    return bw_first, bw_min
+
+
 def build_problem(profile_data: Dict, gpu_cluster, model_config, gbs: int, max_tp: int, max_bs: int,
                   node_sequences: Sequence[Sequence], norm_lc: Optional[Sequence[float]] = None,
                   corrected: Sequence[str] = ()) -> FlatProblem:
@@ -145,20 +165,13 @@ def build_problem(profile_data: Dict, gpu_cluster, model_config, gbs: int, max_t
         layer_compute[i, :len(lc)] = lc
         layer_memory[i, :len(mem)] = mem
 
-    type_memory, bw_first, bw_min = [], [], []
-    node_ids = list(gpu_cluster.nodes.keys())
+    type_memory = []
     for name in type_names:
         mem = gpu_cluster.get_device_memory_for_device_type(name)
         if mem is None:
             raise TypeError("unsupported operand type(s) for *: 'NoneType' and 'int'")   # device_group.py:99-100
         type_memory.append(float(mem))
-        mine = [i for i in node_ids if _type_name(gpu_cluster.nodes[i].device_type) == name]
-        bw_first.append(float(gpu_cluster.get_intra_bandwidth(mine[0])))     # cluster_bandwidth.py:49-54
-        if 'Q2' in corrected:
-            bw_min.append(float(min(gpu_cluster.nodes_info[gpu_cluster.host_entries[i]['ip']]['inter_bandwidth']
-                                    for i in mine)))
-        else:
-            bw_min.append(float(min(gpu_cluster.get_inter_bandwidth(i) for i in mine)))   # :56-68 (Q2)
+    bw_first, bw_min = cluster_bandwidths(gpu_cluster, type_names, corrected)
     uniform_bw = int(len(set(bw_first + bw_min)) == 1)
 
     seqs = [tuple(_type_name(t) for t in seq) for seq in node_sequences]

@@ -94,7 +94,8 @@ SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 
            'metis_enum_device_group_tables', 'metis_sort_workspace_bytes', 'metis_sort_records',
            'metis_enum_compositions', 'metis_generate_rows', 'metis_list_workspace_bytes', 'metis_list_stages',
            'metis_list_window', 'metis_het_search_headroom', 'metis_headroom_workspace_bytes', 'metis_headroom_select',
-           'metis_headroom_front', 'metis_het_search_outputs']
+           'metis_headroom_front', 'metis_het_search_outputs', 'metis_het_recost', 'metis_recost_regret_workspace_bytes',
+           'metis_recost_regret']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -149,6 +150,15 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_het_breakdown.restype = C.c_int
     lib.metis_het_breakdown.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.c_void_p, C.c_int64,
                                         C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.metis_het_recost.restype = C.c_int
+    lib.metis_het_recost.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.c_void_p, C.c_int64,
+                                     C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
+                                     C.c_void_p]
+    lib.metis_recost_regret_workspace_bytes.restype = C.c_int64
+    lib.metis_recost_regret_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
+    lib.metis_recost_regret.restype = C.c_int
+    lib.metis_recost_regret.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_void_p]
     lib.metis_homo_breakdown.restype = C.c_int
     lib.metis_homo_breakdown.argtypes = [C.POINTER(MetisProblem), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
                                          C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

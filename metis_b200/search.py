@@ -517,6 +517,17 @@ class Candidates:
             raw, stages = het_breakdown(lib, p, sp, ws, self.records[idx], dev, per_stage)
         return Breakdown.from_raw(raw, stages)
 
+    def recost(self, bandwidths: np.ndarray) -> 'Recost':
+        """Every candidate under the bandwidth scenarios ``bandwidths`` (float64 [K, 2, num_types]: bw_first, bw_min per
+        type), from the detail rows and device-group rows this object keeps, on this object's own tables."""
+        t0 = time.perf_counter()
+        lib, p, sp, ws, dev, _keep = self._bound()
+        with torch.cuda.device(dev):
+            detail = self._detail_dev if self._detail_dev is not None else torch.from_numpy(self._detail).to(dev)
+            bw = torch.from_numpy(np.ascontiguousarray(bandwidths, dtype=np.float64)).to(dev)
+            costs = het_recost(lib, p, sp, ws, self.records, detail, bw, dev)
+        return finish_recost(self, costs, None, dev, t0)
+
     def _bound(self):
         """This object's problem tables and plan space on the device: (lib, problem struct, space struct, workspace,
         device, the tensors the structs point into)."""
@@ -700,6 +711,143 @@ def het_breakdown(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.
     back = np.empty(n, dtype=np.int64)
     back[order] = np.arange(n)
     return raw[back], (stages[back] if per_stage else None)
+
+
+_RECOST_CHUNK = 1 << 20                   # records per metis_het_recost launch of a windowed result
+
+
+def het_recost(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.ndarray, detail: torch.Tensor,
+               bandwidths: torch.Tensor, device) -> torch.Tensor:
+    """metis_het_recost of ``records`` (host MetisRecord rows) with their detail rows (device uint8 [n, stride]) under
+    the scenarios ``bandwidths`` (device float64 [K, 2, num_types]) on the bound problem / space; returns the device
+    costs [K, n].  Asynchronous on the current stream."""
+    n, K = len(records), int(bandwidths.shape[0])
+    with torch.cuda.device(device):
+        costs = torch.empty((K, n), dtype=torch.float64, device=device)
+        if n == 0:
+            return costs
+        d_rec = torch.from_numpy(np.ascontiguousarray(records).view(np.uint8).reshape(-1).copy()).to(device)
+        s = torch.cuda.current_stream(device)
+        rc = lib.metis_het_recost(C.byref(p_struct), C.byref(s_struct), C.c_void_p(d_rec.data_ptr()), C.c_int64(n),
+                                  C.c_void_p(detail.data_ptr()), C.c_int32(detail.shape[1]),
+                                  C.c_void_p(bandwidths.data_ptr()), C.c_int32(K), C.c_void_p(costs.data_ptr()),
+                                  C.c_void_p(workspace.data_ptr()), C.c_int64(workspace.numel()),
+                                  C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_het_recost')
+    return costs
+
+
+def recost_regret(costs: torch.Tensor) -> Tuple[np.ndarray, np.ndarray]:
+    """metis_recost_regret of the device costs [K, n]: (best [K], regret [n]) on the host."""
+    K, n = int(costs.shape[0]), int(costs.shape[1])
+    lib = native.load_library()
+    dev = costs.device
+    with torch.cuda.device(dev):
+        best = torch.empty(K, dtype=torch.float64, device=dev)
+        regret = torch.empty(max(n, 1), dtype=torch.float64, device=dev)
+        ws = torch.empty(int(lib.metis_recost_regret_workspace_bytes(C.c_int32(K), C.c_int64(n))), dtype=torch.uint8,
+                         device=dev)
+        s = torch.cuda.current_stream(dev)
+        rc = lib.metis_recost_regret(C.c_void_p(costs.data_ptr()), C.c_int32(K), C.c_int64(n), C.c_void_p(best.data_ptr()),
+                                     C.c_void_p(regret.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_int64(ws.numel()),
+                                     C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_recost_regret')
+        return best.cpu().numpy(), regret[:n].cpu().numpy()
+
+
+def stable_cost_order(records: np.ndarray, cost: np.ndarray, device) -> np.ndarray:
+    """Positions of ``records`` (in estimate_costs order) by ascending ``cost``, ties in that order: the existing
+    metis_sort_records(METIS_SORT_BY_COST_STABLE) on a copy of the records whose cost field holds ``cost``."""
+    n = len(records)
+    if n == 0:
+        return np.zeros(0, dtype=np.int64)
+    rows = np.array(records)
+    rows['cost'] = cost
+    lib = native.load_library()
+    with torch.cuda.device(device):
+        buf = torch.from_numpy(rows.view(np.uint8).reshape(-1).copy()).to(device)
+        ws = torch.empty(int(lib.metis_sort_workspace_bytes(C.c_int64(n))), dtype=torch.uint8, device=device)
+        perm = torch.empty(n, dtype=torch.int32, device=device)
+        s = torch.cuda.current_stream(device)
+        rc = lib.metis_sort_records(C.c_void_p(buf.data_ptr()), C.c_int64(n), C.c_int32(native.SORT_BY_COST_STABLE),
+                                    C.c_void_p(perm.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_int64(ws.numel()),
+                                    C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_sort_records')
+        return perm.cpu().numpy().view(np.uint32).astype(np.int64)
+
+
+class Recost:
+    """The candidates of one search re-costed under K bandwidth scenarios (HetSearchResult.recost).
+
+    ``costs[j, i]`` is candidate i's HeteroCostEstimator.get_cost under scenario j, candidates in estimate_costs order;
+    bit for bit what a fresh search under that scenario's cluster returns for the same candidate.  ``regret[i]`` is
+    max_j (costs[j, i] - best cost of scenario j), absolute and in fp64 (costs may be negative on rough profiles)."""
+
+    def __init__(self, candidates, costs: np.ndarray, best_costs: np.ndarray, regret: np.ndarray, device,
+                 timings: Dict[str, float]):
+        self.candidates = candidates
+        self.costs = costs                    # float64 [K, N]
+        self.best_costs = best_costs          # float64 [K]: min over the candidates of each scenario (+inf when N == 0)
+        self.regret = regret                  # float64 [N]
+        self.timings = timings
+        self._device = device
+        self._orders: Dict[int, np.ndarray] = {}
+        self._robust: Optional[np.ndarray] = None
+
+    def __len__(self) -> int:
+        return self.costs.shape[0]
+
+    def _scenario(self, j) -> int:
+        j = int(j)
+        K = self.costs.shape[0]
+        if not -K <= j < K:
+            raise IndexError(f'scenario {j} out of range: {K} scenarios')
+        return j % K
+
+    def order(self, j) -> np.ndarray:
+        """Positions of the candidates in scenario j's ranking: by its cost, ties in estimate_costs order."""
+        j = self._scenario(j)
+        if j not in self._orders:
+            self._orders[j] = stable_cost_order(self.candidates.records, self.costs[j], self._device)
+        return self._orders[j]
+
+    def _tuples(self, pos: np.ndarray, cost: np.ndarray) -> List[Tuple]:
+        return [t[:6] + (float(c),) for t, c in zip(self.candidates.tuples(pos), cost[pos])]
+
+    def ranked(self, j, k: Optional[int] = None) -> List[Tuple]:
+        """The first ``k`` (default: all) of ``sorted(candidates, key=cost)`` under scenario j: the reference's 7-tuples
+        with slot 6 holding scenario j's cost."""
+        j = self._scenario(j)
+        pos = self.order(j)
+        if k is not None:
+            pos = pos[:k]
+        return self._tuples(pos, self.costs[j])
+
+    def best(self, j) -> Optional[Tuple]:
+        """The first entry of ranked(j), or None when the search returned no candidate."""
+        top = self.ranked(j, 1)
+        return top[0] if top else None
+
+    def robust(self, k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """The ``k`` candidates of least regret: (positions in estimate_costs order, their regrets), by ascending regret,
+        ties in estimate_costs order."""
+        if int(k) < 0:
+            raise ValueError(f'k must be >= 0, not {k}')
+        if self._robust is None:
+            self._robust = stable_cost_order(self.candidates.records, self.regret, self._device)
+        pos = self._robust[:int(k)]
+        return pos, self.regret[pos]
+
+
+def finish_recost(candidates, costs_dev: torch.Tensor, costs: Optional[np.ndarray], device, t0: float) -> Recost:
+    """Recost of the device costs [K, N] (``costs``: their host copy when the caller has it), with the regret.
+    timings: ``recost_s`` up to the costs on the host, ``regret_s`` the regret kernels and their copy."""
+    if costs is None:
+        costs = costs_dev.cpu().numpy()
+    t1 = time.perf_counter()
+    best, regret = recost_regret(costs_dev)
+    t2 = time.perf_counter()
+    return Recost(candidates, costs, best, regret, device, {'recost_s': t1 - t0, 'regret_s': t2 - t1})
 
 
 def materialize(records: np.ndarray, detail: np.ndarray, space: flatten.FlatPlanSpace,
@@ -1066,6 +1214,27 @@ class WindowedCandidates:
             for k, t in zip(at.tolist(), got):
                 out[k] = t
         return out
+
+    def recost(self, bandwidths: np.ndarray) -> 'Recost':
+        """Candidates.recost window by window: the detail rows of a window's records come from replaying them
+        (metis_het_detail, like tuples()), their costs go to the host ([K, N] float64)."""
+        t0 = time.perf_counter()
+        n, K = len(self.records), len(bandwidths)
+        costs = np.empty((K, n), dtype=np.float64)
+        dev = self.searcher.dp.device
+        bw = torch.from_numpy(np.ascontiguousarray(bandwidths, dtype=np.float64)).to(dev)
+        for w in range(len(self.windows)):
+            for lo in range(int(self.firsts[w]), int(self.firsts[w + 1]), _RECOST_CHUNK):
+                hi = min(int(self.firsts[w + 1]), lo + _RECOST_CHUNK)
+                rec = self.records[lo:hi]
+                dp = self._load(w)
+                with torch.cuda.device(dev):
+                    detail = torch.from_numpy(self.searcher.detail_for(rec)).to(dev)
+                    costs[:, lo:hi] = het_recost(dp.lib, dp.p_struct, dp.s_struct, self.searcher.workspace, rec, detail,
+                                                 bw, dev).cpu().numpy()
+        with torch.cuda.device(dev):
+            costs_dev = torch.from_numpy(costs).to(dev)
+        return finish_recost(self, costs_dev, costs, dev, t0)
 
     def breakdown(self, idx, per_stage: bool = True) -> Breakdown:
         """Cost terms and memory headroom of the candidates ``idx``, window by window like tuples()."""

@@ -12,7 +12,7 @@ import hashlib
 import json
 import os
 import random
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import Dict, List, Sequence, Tuple
 
 # relative per-layer time of each device type (A100 == 1.0)
@@ -311,6 +311,15 @@ WORKLOADS: Dict[str, Workload] = {w.name: w for w in [
              zero_fb_sync=(('H100', 2, 1),), missing=(('H100', 4, 8),), int_memory=('H100',), seed=108,
              profile_style='rough'),
 ]}
+
+# The same problems under bandwidths that differ by device type (the clusterfile holds one intra_bandwidth per IP, and
+# a Workload gives every node of a type the same IP, so a per-node difference within a type cannot be written here).
+# Bandwidth enters only the cost model: these searches visit the candidates of their base workload, with other costs
+# (HetSearchResult.recost, tests/test_recost.py).  They differ from the base only in intra_bw.
+WORKLOADS.update({w.name: w for w in [
+    replace(WORKLOADS['mix32'], name='bw_mix32', intra_bw={'A100': 2.5e9, 'H100': 9.0e10}),
+    replace(WORKLOADS['rough_t3'], name='bw_rough_t3', intra_bw={'A100': 1.25e9, 'H100': 4.0e10, 'V100': 7.5e8}),
+]})
 
 
 def sweep_workload(ndev: int, ntypes: int, variance: int = 1, mpl: int = 4, num_layers: int = 96,
