@@ -498,25 +498,13 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
         if len(windows) == 1:                                 # one search: the window is the whole space
             space, windows = windows[0].space, None
     t1 = time.perf_counter()
-    if windows is not None:
-        result = _cost_het_windows(problem, space, windows, seqs, dev, rank, world, dist, corrected, t0, t1, headroom,
-                                   misses)
-        result.summary['listing'] = 'host' if listing is None else 'device'
-        result._searched = cluster_signature(gpu_cluster, problem.type_names)
-        return result
-    stride = 3 * int(space.blocks['num_stage'].max()) + 1
-    dp, searcher = _engine(problem, space, dev, rank, world, stride)
-    searcher.want_headroom = headroom
-    if not headroom:
-        searcher.headroom = None
-    searcher.want_misses = misses
-    if not misses:
-        searcher.misses, searcher.miss_capacity = None, 0
-    dp.upload()
-    failure = None
-    out = best = None
+    if windows is None:
+        run, gather, candidates = _one_search(problem, space, seqs, dev, rank, world, headroom, misses)
+    else:
+        run, gather, candidates = _window_search(problem, windows, seqs, dev, rank, world, headroom, misses)
+    failure = out = None
     try:
-        out = searcher.run()
+        out = run()
     except Exception as exc:                                  # noqa: BLE001 - re-raised below on every rank
         if not dist:
             raise
@@ -524,7 +512,7 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     if dist:
         # a rank whose search raised must not leave the others waiting in a collective
         summary, best = search.global_exchange(out.summary if out is not None else {}, out.best if out is not None else None,
-                                               dp.device, int(failure is not None))
+                                               dev, int(failure is not None))
         if summary['any_rank_failed']:
             raise failure if failure is not None else native.MetisNativeError('the search failed on another rank')
         if summary['global_fatal_ordinal'] < 2 ** 62:
@@ -532,35 +520,70 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
                            fatal_aux=summary['global_fatal_aux'])
         else:
             summary['fatal_ordinal'] = 2 ** 64 - 1
-            out = search.gather_records(out, searcher, want_rank=False, counts=summary['records_per_rank'])
+            out = gather(out, summary['records_per_rank'])
             if misses:
                 summary['num_oom_attempts'] = len(out.misses)
     else:
         summary, best = out.summary, out.best
-    if summary['fatal_ordinal'] != 2 ** 64 - 1:
-        # the reference dies at that plan: nothing is returned (quirk Q8)
-        search.raise_fatal(summary, problem)
+    # the reference dies at the first failing plan: nothing is returned (quirk Q8)
+    search.raise_fatal(summary, problem)
     t2 = time.perf_counter()
-    # the row blob of the engine is rewritten by the next call: a lazy result keeps its own copy (a few MB, on the GPU)
-    cand = search.Candidates(out.records, out.detail, space, seqs, detail_dev=out.detail_dev,
-                             rows_dev=dp.rows_device().clone(), problem=problem,
-                             headroom=np.array(out.headroom) if headroom else None,
-                             misses=out.misses if misses else None)   # a fresh array (HetSearcher.run)
+    summary = dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)),
+                   num_windows=len(windows) if windows is not None else 1,
+                   listing='host' if listing is None else 'device')
+    cand, ranker = candidates(out, summary)
     # sorted(result, key=cost) is the CALLER's step in the reference (cost_het_cluster.py:76): its permutation is
     # computed by the device sort when ranked() is first asked for; best() needs no sort at all
-    result = HetSearchResult(cand, out.rank_order,
-                             dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)), num_windows=1,
-                                  listing='host' if listing is None else 'device'),
-                             ranker=search.make_ranker(searcher, out.records_dev) if len(out.records) else None,
-                             best_key=(best[1], best[2]) if best else None)
+    result = HetSearchResult(cand, None, summary, ranker=ranker, best_key=(best[1], best[2]) if best else None)
     result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
                       'decode_columns_s': time.perf_counter() - t2}
-    result._searched = cluster_signature(gpu_cluster, problem.type_names)
     if headroom:
         result.timings['headroom_s'] = out.headroom_s
     if misses:
         result.timings['misses_s'] = out.misses_s
+    result._searched = cluster_signature(gpu_cluster, problem.type_names)
     return result
+
+
+def _one_search(problem, space, seqs, dev, rank: int, world: int, headroom: bool, misses: bool):
+    """The space in one metis_het_search on the cached engine: (search, multi-rank gather of its output, (output,
+    summary) -> (candidates, ranker)).  The candidates keep the detail rows on the device."""
+    from . import search
+    stride = 3 * int(space.blocks['num_stage'].max()) + 1
+    dp, searcher = _engine(problem, space, dev, rank, world, stride)
+    searcher.set_outputs(headroom, misses)
+    dp.upload()
+
+    def gather(out, counts):
+        return search.gather_records(out, searcher, want_rank=False, counts=counts)
+
+    def candidates(out, summary):
+        # the row blob of the engine is rewritten by the next call: a lazy result keeps its own copy (a few MB, on the GPU)
+        cand = search.Candidates(out.records, out.detail, space, seqs, detail_dev=out.detail_dev,
+                                 rows_dev=dp.rows_device().clone(), problem=problem,
+                                 headroom=np.array(out.headroom) if headroom else None,   # the pinned buffer is reused
+                                 misses=out.misses if misses else None)   # a fresh array (HetSearcher.run)
+        return cand, search.make_ranker(searcher, out.records_dev) if len(out.records) else None
+    return searcher.run, gather, candidates
+
+
+def _window_search(problem, windows, seqs, dev, rank: int, world: int, headroom: bool, misses: bool):
+    """cost_het_cluster() for a space larger than one search: flatten.plan_windows' windows, searched in ordinal order
+    (search.search_windows), merged on the host.  Returns like _one_search; the candidates keep the records only
+    (search.WindowSegment)."""
+    from . import search
+    searcher = None
+
+    def run():
+        nonlocal searcher
+        merged, _dp, searcher = search.search_windows(problem, windows, dev, rank, world, headroom=headroom,
+                                                      misses=misses)
+        return merged
+
+    def candidates(merged, summary):
+        cand = search.window_candidates(merged, windows, problem, seqs, searcher)
+        return cand, search.make_window_ranker(searcher, merged.records, summary) if len(merged.records) else None
+    return run, (lambda merged, _counts: search.gather_window_records(merged, dev)), candidates
 
 
 # A space whose search needs less device memory than this (and is within the 32-bit limits of one search) is searched
@@ -653,53 +676,6 @@ def _het_windows(problem, space, dev, rank: int, world: int, num_recs: Optional[
     if plan is not None:
         return plan(budget, per_plan / world, per_row, per_rec)
     return flatten.plan_windows(space, budget, per_plan / world, per_row, per_rec)
-
-
-def _cost_het_windows(problem, space, windows, seqs, dev, rank: int, world: int, dist, corrected, t0: float,
-                      t1: float, headroom: bool = False, misses: bool = False) -> HetSearchResult:
-    """cost_het_cluster() for a space larger than one search: flatten.plan_windows' windows, searched in ordinal order
-    (search.search_windows), merged on the host; the result keeps the records only (search.WindowedCandidates)."""
-    from . import search
-    failure = merged = searcher = None
-    try:
-        merged, _dp, searcher = search.search_windows(problem, windows, dev, rank, world, headroom=headroom,
-                                                      misses=misses)
-    except Exception as exc:                                  # noqa: BLE001 - re-raised below on every rank
-        if not dist:
-            raise
-        failure = exc
-    if dist:
-        summary, best = search.global_exchange(merged.summary if merged is not None else {},
-                                               merged.best if merged is not None else None, dev, int(failure is not None))
-        if summary['any_rank_failed']:
-            raise failure if failure is not None else native.MetisNativeError('the search failed on another rank')
-        if summary['global_fatal_ordinal'] < 2 ** 62:
-            summary.update(fatal_ordinal=summary['global_fatal_ordinal'], fatal_code=summary['global_fatal_code'],
-                           fatal_aux=summary['global_fatal_aux'])
-        else:
-            summary['fatal_ordinal'] = 2 ** 64 - 1
-            merged = search.gather_window_records(merged, dev)
-            if misses:
-                summary['num_oom_attempts'] = len(merged.misses)
-    else:
-        summary, best = merged.summary, merged.best
-    if summary['fatal_ordinal'] != 2 ** 64 - 1:
-        search.raise_fatal(summary, problem)                  # the reference dies at that plan (quirk Q8)
-    t2 = time.perf_counter()
-    cand = search.WindowedCandidates(merged.records, merged.bases, merged.firsts, windows, problem, seqs, searcher,
-                                     headroom=merged.headroom, misses=merged.misses)
-    result = HetSearchResult(cand, None, dict(summary, num_plans=space.num_plans, corrected=tuple(sorted(corrected)),
-                                              num_windows=len(windows)),
-                             best_key=(best[1], best[2]) if best else None)
-    if len(merged.records):
-        result._ranker = search.make_window_ranker(searcher, merged.records, result.summary)
-    result.timings = {'flatten_enumerate_s': t1 - t0, 'gpu_search_s': t2 - t1,
-                      'decode_columns_s': time.perf_counter() - t2}
-    if headroom:
-        result.timings['headroom_s'] = merged.headroom_s
-    if misses:
-        result.timings['misses_s'] = merged.misses_s
-    return result
 
 
 def cost_homo_cluster(args: argparse.Namespace, gpu_cluster, cost_estimator: HomoCostEstimator,

@@ -30,6 +30,52 @@ def _align(n: int, a: int = 256) -> int:
     return (n + a - 1) // a * a
 
 
+def upload(a: np.ndarray, device) -> torch.Tensor:
+    """A copy of the bytes of ``a`` on ``device`` (flat uint8)."""
+    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).to(device)
+
+
+def bind_problem(problem: flatten.FlatProblem, device, space: Optional[flatten.FlatPlanSpace] = None,
+                 rows: Optional[torch.Tensor] = None):
+    """``problem``'s tables (and ``space``'s blocks and batches, with ``rows``, its device-group rows on ``device``)
+    uploaded to ``device``: (lib, problem struct, space struct or None, a workspace for the replay kernels, the tensors
+    the structs point into)."""
+    lib = native.load_library()
+    with torch.cuda.device(device):
+        tens = {k: upload(v, device) for k, v in problem.arrays.items()}
+        if space is not None:
+            tens.update(blocks=upload(space.blocks, device), batches=upload(space.batches, device), rows=rows)
+        p = problem.as_struct(lambda n: tens[n].data_ptr())
+        sp = space.as_struct(lambda n: tens[n].data_ptr()) if space is not None else None
+        ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=device)
+    return lib, p, sp, ws, tens
+
+
+def device_sort(buf: torch.Tensor, n: int, mode: int, stream: torch.cuda.Stream, want_perm: bool = False,
+                workspace: Optional[torch.Tensor] = None) -> Tuple[Optional[torch.Tensor], torch.Tensor]:
+    """metis_sort_records on the first n rows of ``buf`` (device, in place, asynchronous on ``stream``): (the
+    permutation as int32 [n] (a view of the uint32 indices) when asked, else None; the workspace, ``workspace`` when it
+    is large enough, so that a caller can keep it for the next sort)."""
+    lib = native.load_library()
+    need = int(lib.metis_sort_workspace_bytes(C.c_int64(n)))
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need + need // 8, dtype=torch.uint8, device=buf.device)
+    perm = torch.empty(max(n, 1), dtype=torch.int32, device=buf.device) if want_perm else None
+    rc = lib.metis_sort_records(C.c_void_p(buf.data_ptr()), C.c_int64(n), C.c_int32(mode),
+                                C.c_void_p(perm.data_ptr() if perm is not None else 0),
+                                C.c_void_p(workspace.data_ptr()), C.c_int64(workspace.numel()),
+                                C.c_void_p(stream.cuda_stream))
+    native.check(rc, 'metis_sort_records')
+    return (perm[:n] if perm is not None else None), workspace
+
+
+def sorted_positions(rows: np.ndarray, mode: int, device) -> np.ndarray:
+    """Positions of the 16-byte ``rows`` (MetisRecord or MetisMiss) in metis_sort_records(``mode``) order (int64)."""
+    with torch.cuda.device(device):
+        perm, _ws = device_sort(upload(rows, device), len(rows), mode, torch.cuda.current_stream(device), True)
+        return perm.cpu().numpy().view(np.uint32).astype(np.int64)
+
+
 _PROBLEM_ARRAYS = ('key_index', 'layer_compute', 'layer_memory', 'exec_full', 'fb_sync', 'norm_lc', 'type_memory',
                    'type_bw_first', 'type_bw_min', 'ns_run_type', 'ns_run_end', 'ns_q10_end')
 # 'rows' is last: spaces whose rows the GPU writes itself (flatten.build_plan_space(device_rows=True)) upload
@@ -219,8 +265,8 @@ class HetSearcher:
                  want_records: bool = True, want_detail: bool = False, capacity: Optional[int] = None,
                  want_ranking: bool = False, detail_to_host: bool = True, detail_stride: Optional[int] = None,
                  want_headroom: bool = False, want_misses: bool = False):
-        """``want_headroom``: the search also writes each record's memory headroom (metis_het_search_headroom).
-        ``want_misses``: and every out-of-memory partition attempt (metis_het_search_outputs)."""
+        """``want_headroom``: the search also writes each record's memory headroom; ``want_misses``: and every
+        out-of-memory partition attempt (both side outputs of metis_het_search_outputs)."""
         self.dp = dp
         self.want_misses = want_misses
         self.misses = None                                   # int64 [2 * miss_capacity]: MetisMiss rows
@@ -279,6 +325,24 @@ class HetSearcher:
         with torch.cuda.device(self.dp.device):
             self.misses = torch.empty(capacity * 2, dtype=torch.int64, device=self.dp.device)
 
+    def set_outputs(self, headroom: bool, misses: bool) -> None:
+        """Which side outputs the next searches write: each record's memory headroom, every out-of-memory partition
+        attempt.  The buffers of an output no longer written are freed."""
+        self.want_headroom = headroom and self.want_records
+        if not self.want_headroom:
+            self.headroom = None
+        self.want_misses = misses
+        if not misses:
+            self.misses, self.miss_capacity = None, 0
+
+    def release(self) -> None:
+        """Free the search buffers, keeping only what replaying picks needs (metis_het_detail's workspace): what a
+        windowed result holds on to while it is alive."""
+        self.records = self.workspace = self.headroom = self.misses = None
+        self.capacity = self.miss_capacity = 0
+        with torch.cuda.device(self.dp.device):
+            self.workspace = torch.empty(self.dp.workspace_bytes(0), dtype=torch.uint8, device=self.dp.device)
+
     def launch(self, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Enqueue pack + search + finalize + summary copy on ``stream`` (asynchronous)."""
         dp = self.dp
@@ -288,23 +352,17 @@ class HetSearcher:
         if self.want_headroom and self.records is not None and self.headroom is None:
             with torch.cuda.device(dp.device):
                 self.headroom = torch.empty(self.capacity, dtype=torch.float64, device=dp.device)
-        common = (C.c_void_p(self.records.data_ptr() if self.records is not None else 0), C.c_int64(self.capacity),
-                  C.c_void_p(self.detail.data_ptr() if self.detail is not None else 0), C.c_int32(self.detail_stride))
-        tail = (C.c_void_p(self.workspace.data_ptr()), C.c_int64(self.workspace.numel()),
-                C.c_void_p(self.summary_host.data_ptr()), C.c_void_p(s.cuda_stream))
-        if self.want_misses:
-            rc = dp.lib.metis_het_search_outputs(
-                C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard), *common,
-                C.c_void_p(self.headroom.data_ptr() if self.want_headroom else 0), C.c_void_p(self.misses.data_ptr()),
-                C.c_int64(self.miss_capacity), *tail)
-            native.check(rc, 'metis_het_search_outputs')
-        elif self.want_headroom:
-            rc = dp.lib.metis_het_search_headroom(C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard),
-                                                  *common, C.c_void_p(self.headroom.data_ptr()), *tail)
-            native.check(rc, 'metis_het_search_headroom')
-        else:
-            rc = dp.lib.metis_het_search(C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard), *common, *tail)
-            native.check(rc, 'metis_het_search')
+        headroom = self.headroom if self.want_headroom else None
+        misses = self.misses if self.want_misses else None
+        rc = dp.lib.metis_het_search_outputs(
+            C.byref(dp.p_struct), C.byref(dp.s_struct), C.byref(self.shard),
+            C.c_void_p(self.records.data_ptr() if self.records is not None else 0), C.c_int64(self.capacity),
+            C.c_void_p(self.detail.data_ptr() if self.detail is not None else 0), C.c_int32(self.detail_stride),
+            C.c_void_p(headroom.data_ptr() if headroom is not None else 0),
+            C.c_void_p(misses.data_ptr() if misses is not None else 0),
+            C.c_int64(self.miss_capacity if misses is not None else 0), C.c_void_p(self.workspace.data_ptr()),
+            C.c_int64(self.workspace.numel()), C.c_void_p(self.summary_host.data_ptr()), C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_het_search_outputs')
 
     def summary(self) -> native.MetisSearchSummary:
         return native.MetisSearchSummary.from_buffer_copy(self.summary_host.numpy().tobytes())
@@ -405,20 +463,11 @@ class HetSearcher:
                                headroom_dev, headroom_s, misses, misses_s)
 
     def sort_records(self, n: int, mode: int, stream: torch.cuda.Stream, want_perm: bool = False, buf=None):
-        """metis_sort_records on the first n records (device, in place, asynchronous on ``stream``); returns the
-        permutation tensor (int32 view of the uint32 indices) when asked."""
-        dp = self.dp
-        need = int(dp.lib.metis_sort_workspace_bytes(C.c_int64(n)))
-        if self._sort_ws is None or self._sort_ws.numel() < need:
-            self._sort_ws = torch.empty(need + need // 8, dtype=torch.uint8, device=dp.device)
-        perm = torch.empty(max(n, 1), dtype=torch.int32, device=dp.device) if want_perm else None
-        buf = self.records if buf is None else buf
-        rc = dp.lib.metis_sort_records(C.c_void_p(buf.data_ptr()), C.c_int64(n), C.c_int32(mode),
-                                       C.c_void_p(perm.data_ptr() if perm is not None else 0),
-                                       C.c_void_p(self._sort_ws.data_ptr()), C.c_int64(self._sort_ws.numel()),
-                                       C.c_void_p(stream.cuda_stream))
-        native.check(rc, 'metis_sort_records')
-        return perm[:n] if perm is not None else None
+        """device_sort of the first n records of ``buf`` (default: the record buffer), with the sort workspace kept
+        for the next sort; returns the permutation when asked."""
+        perm, self._sort_ws = device_sort(self.records if buf is None else buf, n, mode, stream, want_perm,
+                                          self._sort_ws)
+        return perm
 
     def detail_for(self, picks: np.ndarray, stream: Optional[torch.cuda.Stream] = None) -> np.ndarray:
         """Strategies and partition of chosen records (metis_het_detail replay)."""
@@ -426,7 +475,7 @@ class HetSearcher:
         s = stream or torch.cuda.current_stream(dp.device)
         n = len(picks)
         with torch.cuda.device(dp.device):
-            raw = torch.from_numpy(np.ascontiguousarray(picks).view(np.uint8).reshape(-1).copy()).to(dp.device)
+            raw = upload(picks, dp.device)
             out = torch.zeros((max(n, 1), native.DETAIL_STRIDE), dtype=torch.uint8, device=dp.device)
             rc = dp.lib.metis_het_detail(C.byref(dp.p_struct), C.byref(dp.s_struct), C.c_void_p(raw.data_ptr()),
                                          C.c_int64(n), C.c_void_p(out.data_ptr()), C.c_int32(native.DETAIL_STRIDE),
@@ -458,138 +507,251 @@ class Candidates:
     """Vectorised view of the costed candidates: every column of the reference's 7-tuples
     (cost_het_cluster.py:44-46) as a numpy array, the tuples themselves built on demand.
 
-    ``detail`` rows hold dp codes[S], tp codes[S] (log2) and layer_partition[S+1]; they may still be on the device
-    (``detail_dev``): rows are then fetched per request (a ranked slice costs one small gather + copy), or all at
-    once the first time more than a few thousand are needed."""
+    The records (host, estimate_costs order) are split into segments: the records [first, end) of one plan space,
+    whose ordinals are global ordinals less the segment's ``base``.  One search is one SearchSegment at base 0, a
+    windowed search one WindowSegment per window.  A segment binds its tables on the device and gives its records'
+    detail rows (dp codes[S], tp codes[S] (log2) and layer_partition[S+1]); every view below splits its request by
+    segment (``_split``)."""
 
-    _BULK = 4096
-
-    def __init__(self, records: np.ndarray, detail: Optional[np.ndarray], space: flatten.FlatPlanSpace,
+    def __init__(self, records: np.ndarray, detail: Optional[np.ndarray], space: Optional[flatten.FlatPlanSpace],
                  node_sequences: Sequence[Tuple], detail_dev: Optional[torch.Tensor] = None,
                  rows_dev: Optional[torch.Tensor] = None, problem: Optional[flatten.FlatProblem] = None,
-                 headroom: Optional[np.ndarray] = None, misses: Optional[np.ndarray] = None):
+                 headroom: Optional[np.ndarray] = None, misses: Optional[np.ndarray] = None,
+                 segments: Optional[Sequence] = None):
+        """The candidates of one search (a SearchSegment of ``space`` with the search's ``detail`` / ``detail_dev``
+        rows and ``rows_dev`` device-group rows, replayed on ``problem``), or, given ``segments``, records split into
+        those (a windowed search: window_candidates)."""
         self.records = records
-        self.misses = misses                  # MISS_HOST_DTYPE in reference order (a search with misses), else None
+        self.misses = misses                  # MISS_HOST_DTYPE, global ordinals, reference order; else None
         self.headroom = headroom              # float64 per record (a search with headroom), else None
-        self.device = rows_dev.device if rows_dev is not None else None   # where the search ran (None: not known)
-        self.space = space
-        self.problem = problem                # the tables breakdown() replays the candidates on
+        self.space = space                    # the plan space of a one-search result; None for segments
+        if segments is None:
+            segments = [SearchSegment(space, len(records), problem, detail, detail_dev, rows_dev)]
+        self.segments = list(segments)
+        self.device = self.segments[0].device     # where the search ran (None: not known)
+        self.problem = self.segments[0].problem   # the tables the candidates are replayed on
         self.node_sequences = [tuple(s) for s in node_sequences]
+        self.cost = records['cost']
+        self.bases = np.asarray([s.base for s in self.segments], dtype=np.int64)
+        self.firsts = np.asarray([s.first for s in self.segments] + [self.segments[-1].end], dtype=np.int64)
+
+    def __len__(self) -> int:
+        return len(self.records)
+
+    @property
+    def windows(self) -> list:
+        """The windows of a windowed result, in ordinal order."""
+        return [s.window for s in self.segments]
+
+    def _split(self, values: np.ndarray, starts: np.ndarray):
+        """(segment, positions into ``values``) of every segment holding some of ``values``: positions of records
+        (``starts`` = self.firsts) or global ordinals (``starts`` = self.bases)."""
+        seg = np.searchsorted(starts, values, side='right') - 1
+        for s in np.unique(seg).tolist():
+            yield self.segments[s], np.nonzero(seg == s)[0]
+
+    def index_of(self, ordinal: int, step: int) -> Optional[int]:
+        """Position of the candidate (global ordinal, step), or None: bisection over the (ordinal, step)-sorted records
+        of the segment that holds the ordinal."""
+        s = int(np.searchsorted(self.bases, ordinal, side='right')) - 1
+        rel = int(ordinal) - int(self.bases[s]) if s >= 0 else -1
+        if not 0 <= rel <= 0xFFFFFFFF:
+            return None
+        return _bisect_records(self.records, self.segments[s].first, self.segments[s].end, rel, int(step))
+
+    def detail_rows(self, idx) -> np.ndarray:
+        """dp codes[S], tp codes[S] (log2) and layer_partition[S+1] of the candidates ``idx``, uint8 [n, stride]."""
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        got = [(at, seg.detail(idx[at] - seg.first, self.records[idx[at]])) for seg, at in self._split(idx, self.firsts)]
+        out = np.zeros((len(idx), max((d.shape[1] for _, d in got), default=native.DETAIL_STRIDE)), dtype=np.uint8)
+        for at, d in got:
+            out[at, :d.shape[1]] = d
+        return out
+
+    def tuples(self, idx) -> List[Tuple]:
+        """The reference's 7-tuples of the candidates ``idx`` (any integer sequence)."""
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        out: List[Optional[Tuple]] = [None] * len(idx)
+        for seg, at in self._split(idx, self.firsts):
+            rec = self.records[idx[at]]
+            det = seg.detail(idx[at] - seg.first, rec)
+            col = plan_geometry(seg.space, rec['ordinal'])
+            codes = seg.group_codes(col['row_byte'], col['num_stage'])
+            nrep, cost = rec['num_repartition'].astype(np.int64), rec['cost']
+            for k, i in enumerate(at.tolist()):
+                S = int(col['num_stage'][k])
+                d = det[k]
+                groups = (1 << codes[k, :S].astype(np.int64)).tolist()
+                dp = (1 << d[:S].astype(np.int64)).tolist()
+                tp = (1 << d[S:2 * S].astype(np.int64)).tolist()
+                part = d[2 * S:3 * S + 1].astype(np.int64).tolist()
+                out[i] = (self.node_sequences[int(col['ns_idx'][k])], groups, list(zip(dp, tp)), int(col['batches'][k]),
+                          part, int(nrep[k]), float(cost[k]))
+        return out
+
+    def plan_columns(self, ordinals: np.ndarray) -> Dict[str, np.ndarray]:
+        """ns_idx, num_stage, batches and the log2 device-group codes (``codes``, [n, METIS_MAX_STAGES]) of the plans of
+        the global ``ordinals``."""
+        ordinals = np.asarray(ordinals, dtype=np.int64).reshape(-1)
+        n = len(ordinals)
+        out: Dict[str, np.ndarray] = {}
+        for seg, at in self._split(ordinals, self.bases):
+            col = plan_geometry(seg.space, ordinals[at] - seg.base)
+            col['codes'] = seg.group_codes(col['row_byte'], col['num_stage'])
+            for k, v in col.items():
+                if k not in out:
+                    out[k] = np.zeros((n, native.METIS_MAX_STAGES) if k == 'codes' else n, dtype=v.dtype)
+                if k == 'codes':
+                    out[k][at, :v.shape[1]] = v
+                else:
+                    out[k][at] = v
+        return out
+
+    def trace(self, ordinals: np.ndarray) -> List[list]:
+        """verbose.decode_plan of the plans of the global ``ordinals`` (metis_het_trace)."""
+        ordinals = np.asarray(ordinals, dtype=np.int64).reshape(-1)
+        out: List[Optional[list]] = [None] * len(ordinals)
+        for seg, at in self._split(ordinals, self.bases):
+            lib, p, sp, ws, dev, _keep = seg.bind()
+            got = trace_decoded(lib, p, sp, ws, dev, ordinals[at] - seg.base, int(seg.space.blocks['num_stage'].max()))
+            for k, t in zip(at.tolist(), got):
+                out[k] = t
+        return out
+
+    def breakdown(self, idx, per_stage: bool = True) -> Breakdown:
+        """Cost terms and memory headroom of the candidates ``idx`` (metis_het_breakdown)."""
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        width = max(int(self.records['num_stage'][idx].max()), 1) if len(idx) else 1
+        raw = np.zeros(len(idx), dtype=native.BREAKDOWN_DTYPE)
+        stages = np.full((len(idx), native.BD_FIELDS, width), np.nan) if per_stage else None
+        for seg, at in self._split(idx, self.firsts):
+            lib, p, sp, ws, dev, _keep = seg.bind()
+            het_breakdown(lib, p, sp, ws, self.records[idx[at]], dev, at, raw, stages)
+        return Breakdown.from_raw(raw, stages)
+
+    def recost(self, bandwidths: np.ndarray) -> 'Recost':
+        """Every candidate under the bandwidth scenarios ``bandwidths`` (float64 [K, 2, num_types]: bw_first, bw_min per
+        type), _RECOST_CHUNK records per launch, each with its detail rows.  timings: ``recost_s`` up to the costs on
+        the host, ``regret_s`` the regret kernels and their copy."""
+        t0 = time.perf_counter()
+        dev = _require_cuda(self.device)
+        with torch.cuda.device(dev):
+            bw = torch.from_numpy(np.ascontiguousarray(bandwidths, dtype=np.float64)).to(dev)
+            costs_dev = torch.empty((len(bandwidths), len(self.records)), dtype=torch.float64, device=dev)
+            for seg in self.segments:
+                if seg.first == seg.end:                      # nothing to replay: a window is not reloaded for it
+                    continue
+                lib, p, sp, ws, _dev, _keep = seg.bind()
+                for lo in range(seg.first, seg.end, _RECOST_CHUNK):
+                    hi = min(seg.end, lo + _RECOST_CHUNK)
+                    rec = self.records[lo:hi]
+                    detail = seg.detail_device(lo - seg.first, hi - seg.first, rec, dev)
+                    costs_dev[:, lo:hi] = het_recost(lib, p, sp, ws, rec, detail, bw, dev)
+            costs = costs_dev.cpu().numpy()
+        t1 = time.perf_counter()
+        best, regret = recost_regret(costs_dev)
+        t2 = time.perf_counter()
+        return Recost(self, costs, best, regret, dev, {'recost_s': t1 - t0, 'regret_s': t2 - t1})
+
+
+_BULK = 4096           # rows a one-search result gathers on the device per request; more are fetched whole, once
+
+
+def group_codes(rows, row_byte: np.ndarray, stages: np.ndarray) -> np.ndarray:
+    """log2(device count) of every stage of the device-group rows at ``row_byte`` in the row blob ``rows`` (numpy, or a
+    device tensor: gathered there), uint8 [n, max stages] (columns past a row's stage count are junk)."""
+    at = row_byte[:, None] + np.arange(int(stages.max()), dtype=np.int64)[None, :]
+    if isinstance(rows, np.ndarray):
+        return rows[np.minimum(at, len(rows) - 1)]
+    return rows[torch.from_numpy(np.minimum(at, rows.numel() - 1)).to(rows.device)].cpu().numpy()
+
+
+class SearchSegment:
+    """The ``end`` records of one search (base 0) with the detail rows and device-group rows the search kept: host
+    arrays, or device tensors (``detail_dev``, ``rows_dev``) gathered per request (a ranked slice costs one small
+    gather + copy) or fetched whole the first time a request needs more than _BULK rows.  Its tables are bound from
+    this object's own copies, so a later search cannot change what is replayed."""
+
+    base = first = 0
+
+    def __init__(self, space: flatten.FlatPlanSpace, end: int, problem: Optional[flatten.FlatProblem] = None,
+                 detail: Optional[np.ndarray] = None, detail_dev: Optional[torch.Tensor] = None,
+                 rows_dev: Optional[torch.Tensor] = None):
+        self.space = space
+        self.end = end
+        self.problem = problem
+        self.device = rows_dev.device if rows_dev is not None else None
         self._detail = detail
         self._detail_dev = detail_dev
         # device-group rows: the blob the GPU wrote (``rows_dev``, SURVEY.md 8(f)-1) or the host enumerator's
         self._rows_dev = rows_dev
         self._rows = None if rows_dev is not None else space.host_rows()
-        self.cost = records['cost']
 
-    def columns(self, idx=None) -> Dict[str, np.ndarray]:
-        """ns_idx, num_stage, row (dg_idx), batches, num_repartition of the candidates ``idx`` (default: all)."""
-        rec = self.records if idx is None else self.records[idx]
-        return dict(plan_geometry(self.space, rec['ordinal']), num_repartition=rec['num_repartition'].astype(np.int64))
-
-    def group_codes(self, row_byte: np.ndarray, stages: np.ndarray) -> np.ndarray:
-        """log2(device count) of every stage, uint8 [n, max stages] (columns past a row's stage count are junk)."""
-        width = int(stages.max())
-        at = row_byte[:, None] + np.arange(width, dtype=np.int64)[None, :]
-        if self._rows is None:
-            if len(row_byte) > self._BULK:
-                self._rows = self._rows_dev.cpu().numpy()
-                self._rows_dev = None
-            else:
-                sel = torch.from_numpy(np.minimum(at, self._rows_dev.numel() - 1)).to(self._rows_dev.device)
-                return self._rows_dev[sel].cpu().numpy()
-        return self._rows[np.minimum(at, len(self._rows) - 1)]
-
-    def __len__(self) -> int:
-        return len(self.records)
-
-    def index_of(self, ordinal: int, step: int) -> Optional[int]:
-        """Position of the candidate (ordinal, step), or None: bisection over the (ordinal, step)-sorted records."""
-        return _bisect_records(self.records, 0, len(self.records), int(ordinal), int(step))
-
-    def breakdown(self, idx, per_stage: bool = True) -> Breakdown:
-        """Cost terms and memory headroom of the candidates ``idx`` (metis_het_breakdown).  The problem tables and plan
-        space descriptors are uploaded from this object's own copies, so a later search cannot change what is
-        replayed."""
-        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
-        lib, p, sp, ws, dev, _keep = self._bound()
-        with torch.cuda.device(dev):
-            raw, stages = het_breakdown(lib, p, sp, ws, self.records[idx], dev, per_stage)
-        return Breakdown.from_raw(raw, stages)
-
-    def recost(self, bandwidths: np.ndarray) -> 'Recost':
-        """Every candidate under the bandwidth scenarios ``bandwidths`` (float64 [K, 2, num_types]: bw_first, bw_min per
-        type), from the detail rows and device-group rows this object keeps, on this object's own tables."""
-        t0 = time.perf_counter()
-        lib, p, sp, ws, dev, _keep = self._bound()
-        with torch.cuda.device(dev):
-            detail = self._detail_dev if self._detail_dev is not None else torch.from_numpy(self._detail).to(dev)
-            bw = torch.from_numpy(np.ascontiguousarray(bandwidths, dtype=np.float64)).to(dev)
-            costs = het_recost(lib, p, sp, ws, self.records, detail, bw, dev)
-        return finish_recost(self, costs, None, dev, t0)
-
-    def _bound(self):
-        """This object's problem tables and plan space on the device: (lib, problem struct, space struct, workspace,
-        device, the tensors the structs point into)."""
+    def bind(self):
+        """(lib, problem struct, space struct, workspace, device, the tensors the structs point into)."""
         if self.problem is None:
             raise ValueError('these candidates were built without their problem tables: no replay')
-        dev = self._rows_dev.device if self._rows_dev is not None else _require_cuda(None)
-        lib = native.load_library()
-        with torch.cuda.device(dev):
-            tens = {k: torch.from_numpy(np.ascontiguousarray(v).view(np.uint8).reshape(-1).copy()).to(dev)
-                    for k, v in self.problem.arrays.items()}
-            for k in ('blocks', 'batches'):
-                tens[k] = torch.from_numpy(np.ascontiguousarray(getattr(self.space, k)).view(np.uint8).reshape(-1)
-                                           .copy()).to(dev)
-            tens['rows'] = self._rows_dev if self._rows_dev is not None else torch.from_numpy(self._rows).to(dev)
-            p = self.problem.as_struct(lambda n: tens[n].data_ptr())
-            sp = self.space.as_struct(lambda n: tens[n].data_ptr())
-            ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=dev)
+        dev = self.device if self.device is not None else _require_cuda(None)
+        rows = self._rows_dev if self._rows_dev is not None else torch.from_numpy(self._rows).to(dev)
+        lib, p, sp, ws, tens = bind_problem(self.problem, dev, self.space, rows)
         return lib, p, sp, ws, dev, tens
 
-    def plan_columns(self, ordinals: np.ndarray) -> Dict[str, np.ndarray]:
-        """ns_idx, num_stage, batches and the log2 device-group codes of the plans ``ordinals``."""
-        col = plan_geometry(self.space, ordinals)
-        col['codes'] = self.group_codes(col['row_byte'], col['num_stage']) if len(ordinals) else np.zeros((0, 1), np.uint8)
-        return col
-
-    def trace(self, ordinals: np.ndarray) -> List[list]:
-        """verbose.decode_plan of the plans ``ordinals`` (metis_het_trace on this object's own tables)."""
-        lib, p, sp, ws, dev, _keep = self._bound()
-        return trace_decoded(lib, p, sp, ws, dev, ordinals, int(self.space.blocks['num_stage'].max()))
-
-    def detail_rows(self, idx: np.ndarray) -> np.ndarray:
+    def detail(self, pos: np.ndarray, rec: np.ndarray) -> np.ndarray:
+        """Detail rows of the records at ``pos`` (segment positions; ``rec``: those records) on the host."""
         if self._detail is None:
             if self._detail_dev is None:
                 raise ValueError('the search was run without detail rows')
-            if len(idx) > self._BULK:
-                self._detail = self._detail_dev.cpu().numpy()
-                self._detail_dev = None
+            if len(pos) > _BULK:
+                self._detail, self._detail_dev = self._detail_dev.cpu().numpy(), None
             else:
-                sel = torch.from_numpy(np.ascontiguousarray(idx, dtype=np.int64)).to(self._detail_dev.device)
+                sel = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.int64)).to(self._detail_dev.device)
                 return self._detail_dev.index_select(0, sel).cpu().numpy()
-        return self._detail[idx]
+        return self._detail[pos]
 
-    def tuples(self, idx) -> List[Tuple]:
-        """The reference's 7-tuples of the candidates ``idx`` (any integer sequence)."""
-        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
-        if not len(idx):
-            return []
-        det = self.detail_rows(idx)
-        col = self.columns(idx)
-        cost = self.cost[idx]
-        out = []
-        codes = self.group_codes(col['row_byte'], col['num_stage'])
-        for k in range(len(idx)):
-            S = int(col['num_stage'][k])
-            d = det[k]
-            groups = (1 << codes[k, :S].astype(np.int64)).tolist()
-            dp = (1 << d[:S].astype(np.int64)).tolist()
-            tp = (1 << d[S:2 * S].astype(np.int64)).tolist()
-            part = d[2 * S:3 * S + 1].astype(np.int64).tolist()
-            out.append((self.node_sequences[int(col['ns_idx'][k])], groups, list(zip(dp, tp)), int(col['batches'][k]),
-                        part, int(col['num_repartition'][k]), float(cost[k])))
-        return out
+    def detail_device(self, lo: int, hi: int, rec: np.ndarray, device) -> torch.Tensor:
+        """Detail rows of the records [lo, hi) of the segment on ``device``."""
+        if self._detail_dev is not None:
+            return self._detail_dev[lo:hi]
+        return torch.from_numpy(self.detail(np.arange(lo, hi), rec)).to(device)
+
+    def group_codes(self, row_byte: np.ndarray, stages: np.ndarray) -> np.ndarray:
+        if self._rows is None and len(row_byte) > _BULK:
+            self._rows, self._rows_dev = self._rows_dev.cpu().numpy(), None
+        return group_codes(self._rows if self._rows is not None else self._rows_dev, row_byte, stages)
+
+
+class WindowSegment:
+    """The records [first, end) of one window of a windowed search: only the 16 B records are kept.  Device groups,
+    strategies and partitions are rebuilt per request in the search's DeviceProblem / HetSearcher (the arena, sized
+    for the largest window's rows, and metis_het_detail's small workspace stay allocated while the result is alive):
+    the window is reloaded whenever the arena holds something else, its rows regenerated on the device (row kernel)
+    and its picks replayed by metis_het_detail.  The blob is never fetched: only the rows asked for are gathered."""
+
+    def __init__(self, window, first: int, end: int, problem: flatten.FlatProblem, searcher: 'HetSearcher'):
+        self.window = window
+        self.space = window.space
+        self.base, self.first, self.end = int(window.base), int(first), int(end)
+        self.problem = problem
+        self.searcher = searcher
+        self.device = searcher.dp.device
+
+    def bind(self):
+        dp = self.searcher.dp
+        if dp.space is not self.space or dp.problem is not self.problem:
+            dp.reload(self.problem, self.space)               # metis_het_detail needs no more workspace than it has
+            dp.upload()
+        return dp.lib, dp.p_struct, dp.s_struct, self.searcher.workspace, dp.device, None
+
+    def detail(self, pos: np.ndarray, rec: np.ndarray) -> np.ndarray:
+        self.bind()
+        return self.searcher.detail_for(rec)
+
+    def detail_device(self, lo: int, hi: int, rec: np.ndarray, device) -> torch.Tensor:
+        return torch.from_numpy(self.detail(None, rec)).to(device)
+
+    def group_codes(self, row_byte: np.ndarray, stages: np.ndarray) -> np.ndarray:
+        self.bind()
+        return group_codes(self.searcher.dp.rows_device(), row_byte, stages)
 
 
 def plan_geometry(space: flatten.FlatPlanSpace, ordinals: np.ndarray) -> Dict[str, np.ndarray]:
@@ -619,7 +781,7 @@ def trace_decoded(lib, p_struct, s_struct, workspace: torch.Tensor, device, ordi
     while len(todo):
         n = len(todo)
         with torch.cuda.device(device):
-            d_ord = torch.from_numpy(ordinals[todo].view(np.int32).copy()).to(device)
+            d_ord = upload(ordinals[todo], device)
             buf = torch.zeros((max(n, 1), words), dtype=torch.int64, device=device)
             s = torch.cuda.current_stream(device)
             rc = lib.metis_het_trace(C.byref(p_struct), C.byref(s_struct), C.c_void_p(d_ord.data_ptr()), C.c_int64(n),
@@ -680,22 +842,23 @@ class Breakdown:
 _BREAKDOWN_CHUNK = 1 << 16                 # picks per launch: bounds the per-stage buffers of one call
 
 
-def het_breakdown(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.ndarray, device,
-                  per_stage: bool = True, width: Optional[int] = None) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+def het_breakdown(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.ndarray, device, at: np.ndarray,
+                  raw: np.ndarray, stages: Optional[np.ndarray]) -> None:
     """metis_het_breakdown of ``records`` (any order) on the problem / space bound in ``p_struct`` / ``s_struct``:
-    the picks are sorted by (ordinal, step), so that each plan is replayed once, and the rows scattered back to the
-    order given.  Returns (MetisBreakdown rows, per-stage values [n, METIS_BD_FIELDS, width] or None)."""
+    the picks are sorted by (ordinal, step), so that each plan is replayed once, and the row of records[k] is written
+    to raw[at[k]] (MetisBreakdown) and, unless ``stages`` is None, stages[at[k]] (per-stage values
+    [METIS_BD_FIELDS, width])."""
     n = len(records)
     order = np.lexsort((records['step'], records['ordinal']))
     picks = np.ascontiguousarray(records[order])
-    width = int(width or (int(picks['num_stage'].max()) if n else 1))
-    raw = np.zeros(n, dtype=native.BREAKDOWN_DTYPE)
-    stages = np.full((n, native.BD_FIELDS, width), np.nan) if per_stage else None
+    dest = at[order]
+    per_stage = stages is not None
+    width = stages.shape[2] if per_stage else 1
     with torch.cuda.device(device):
         s = torch.cuda.current_stream(device)
         for lo in range(0, n, _BREAKDOWN_CHUNK):
             hi = min(n, lo + _BREAKDOWN_CHUNK)
-            d_picks = torch.from_numpy(picks[lo:hi].view(np.uint8).reshape(-1).copy()).to(device)
+            d_picks = upload(picks[lo:hi], device)
             d_out = torch.empty((hi - lo) * raw.itemsize, dtype=torch.uint8, device=device)
             d_st = torch.empty((hi - lo) * native.BD_FIELDS * width, dtype=torch.float64, device=device) \
                 if per_stage else None
@@ -705,15 +868,12 @@ def het_breakdown(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.
                                          C.c_void_p(workspace.data_ptr()), C.c_int64(workspace.numel()),
                                          C.c_void_p(s.cuda_stream))
             native.check(rc, 'metis_het_breakdown')
-            raw[lo:hi] = d_out.cpu().numpy().view(native.BREAKDOWN_DTYPE)
+            raw[dest[lo:hi]] = d_out.cpu().numpy().view(native.BREAKDOWN_DTYPE)
             if per_stage:
-                stages[lo:hi] = d_st.cpu().numpy().reshape(hi - lo, native.BD_FIELDS, width)
-    back = np.empty(n, dtype=np.int64)
-    back[order] = np.arange(n)
-    return raw[back], (stages[back] if per_stage else None)
+                stages[dest[lo:hi]] = d_st.cpu().numpy().reshape(hi - lo, native.BD_FIELDS, width)
 
 
-_RECOST_CHUNK = 1 << 20                   # records per metis_het_recost launch of a windowed result
+_RECOST_CHUNK = 1 << 20                   # records per metis_het_recost launch: bounds a window's replayed detail rows
 
 
 def het_recost(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.ndarray, detail: torch.Tensor,
@@ -726,7 +886,7 @@ def het_recost(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.nda
         costs = torch.empty((K, n), dtype=torch.float64, device=device)
         if n == 0:
             return costs
-        d_rec = torch.from_numpy(np.ascontiguousarray(records).view(np.uint8).reshape(-1).copy()).to(device)
+        d_rec = upload(records, device)
         s = torch.cuda.current_stream(device)
         rc = lib.metis_het_recost(C.byref(p_struct), C.byref(s_struct), C.c_void_p(d_rec.data_ptr()), C.c_int64(n),
                                   C.c_void_p(detail.data_ptr()), C.c_int32(detail.shape[1]),
@@ -758,22 +918,11 @@ def recost_regret(costs: torch.Tensor) -> Tuple[np.ndarray, np.ndarray]:
 def stable_cost_order(records: np.ndarray, cost: np.ndarray, device) -> np.ndarray:
     """Positions of ``records`` (in estimate_costs order) by ascending ``cost``, ties in that order: the existing
     metis_sort_records(METIS_SORT_BY_COST_STABLE) on a copy of the records whose cost field holds ``cost``."""
-    n = len(records)
-    if n == 0:
+    if len(records) == 0:
         return np.zeros(0, dtype=np.int64)
     rows = np.array(records)
     rows['cost'] = cost
-    lib = native.load_library()
-    with torch.cuda.device(device):
-        buf = torch.from_numpy(rows.view(np.uint8).reshape(-1).copy()).to(device)
-        ws = torch.empty(int(lib.metis_sort_workspace_bytes(C.c_int64(n))), dtype=torch.uint8, device=device)
-        perm = torch.empty(n, dtype=torch.int32, device=device)
-        s = torch.cuda.current_stream(device)
-        rc = lib.metis_sort_records(C.c_void_p(buf.data_ptr()), C.c_int64(n), C.c_int32(native.SORT_BY_COST_STABLE),
-                                    C.c_void_p(perm.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_int64(ws.numel()),
-                                    C.c_void_p(s.cuda_stream))
-        native.check(rc, 'metis_sort_records')
-        return perm.cpu().numpy().view(np.uint32).astype(np.int64)
+    return sorted_positions(rows, native.SORT_BY_COST_STABLE, device)
 
 
 class Recost:
@@ -837,17 +986,6 @@ class Recost:
             self._robust = stable_cost_order(self.candidates.records, self.regret, self._device)
         pos = self._robust[:int(k)]
         return pos, self.regret[pos]
-
-
-def finish_recost(candidates, costs_dev: torch.Tensor, costs: Optional[np.ndarray], device, t0: float) -> Recost:
-    """Recost of the device costs [K, N] (``costs``: their host copy when the caller has it), with the regret.
-    timings: ``recost_s`` up to the costs on the host, ``regret_s`` the regret kernels and their copy."""
-    if costs is None:
-        costs = costs_dev.cpu().numpy()
-    t1 = time.perf_counter()
-    best, regret = recost_regret(costs_dev)
-    t2 = time.perf_counter()
-    return Recost(candidates, costs, best, regret, device, {'recost_s': t1 - t0, 'regret_s': t2 - t1})
 
 
 def materialize(records: np.ndarray, detail: np.ndarray, space: flatten.FlatPlanSpace,
@@ -1027,67 +1165,65 @@ def search_windows(problem: flatten.FlatProblem, windows: Sequence[flatten.PlanW
         if merge.add(w.base, out.summary, out.best, np.array(out.records) if out.records is not None else None,
                      np.array(out.headroom) if out.headroom is not None else None, out.misses):
             break
-    searcher.records = searcher.workspace = searcher.headroom = searcher.misses = None
-    searcher.miss_capacity = 0
-    searcher.capacity = 0
-    with torch.cuda.device(dp.device):
-        searcher.workspace = torch.empty(dp.workspace_bytes(0), dtype=torch.uint8, device=dp.device)
+    searcher.release()
     return merge.result(), dp, searcher
 
 
-def merge_rank_windows(all_counts: np.ndarray, rank_records: Sequence[np.ndarray]) -> Tuple[np.ndarray, np.ndarray]:
-    """The records of every rank -> one list in estimate_costs order.  ``all_counts[r, w]``: records of rank r in
-    window w; ``rank_records[r]``: rank r's records, window by window.  Returns (records, first record per window +
-    total): each window's union ordered by (ordinal, step), windows in order."""
+def window_candidates(merged: WindowedOutput, windows: Sequence, problem: flatten.FlatProblem,
+                      node_sequences: Sequence[Tuple], searcher: HetSearcher) -> Candidates:
+    """The candidates of a windowed search (search_windows' searcher, its merged or gathered output): one WindowSegment
+    per window searched."""
+    segments = [WindowSegment(w, merged.firsts[k], merged.firsts[k + 1], problem, searcher)
+                for k, w in enumerate(windows[:len(merged.bases)])]
+    return Candidates(merged.records, None, None, node_sequences, headroom=merged.headroom, misses=merged.misses,
+                      segments=segments)
+
+
+def merge_rank_windows(all_counts: np.ndarray, records: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+    """The records of every rank -> estimate_costs order.  ``records``: every rank's records, rank after rank, each
+    rank's window by window; ``all_counts[r, w]``: records of rank r in window w.  Returns (positions into ``records``
+    in estimate_costs order: each window's union by (ordinal, step), windows in order; first record per window +
+    total), so that whatever travels with the records follows them by the same positions."""
     world, nwin = all_counts.shape
-    starts = np.concatenate([np.zeros((world, 1), dtype=np.int64), np.cumsum(all_counts, axis=1)], axis=1)
+    starts = np.concatenate([[0], np.cumsum(all_counts.reshape(-1))]).astype(np.int64)    # rank-major
     parts, firsts = [], [0]
     for w in range(nwin):
-        union = np.concatenate([rank_records[r][starts[r, w]:starts[r, w + 1]] for r in range(world)])
-        parts.append(union[np.lexsort((union['step'], union['ordinal']))])
-        firsts.append(firsts[-1] + len(union))
-    rec = np.concatenate(parts) if parts else np.zeros(0, dtype=native.RECORD_DTYPE)
-    return rec, np.asarray(firsts, dtype=np.int64)
+        at = np.concatenate([np.arange(starts[r * nwin + w], starts[r * nwin + w + 1]) for r in range(world)])
+        union = records[at]
+        parts.append(at[np.lexsort((union['step'], union['ordinal']))])
+        firsts.append(firsts[-1] + len(at))
+    return (np.concatenate(parts) if parts else np.zeros(0, dtype=np.int64)), np.asarray(firsts, dtype=np.int64)
 
 
 def gather_window_records(merged: WindowedOutput, device) -> WindowedOutput:
-    """Multi-GPU: every rank receives every rank's records, window by window in estimate_costs order (records only).
-    Two all_gathers on ``device``: the per-window record counts and the padded records; then merge_rank_windows.
-    Every rank must have searched the same windows (no fatal plan: api.cost_het_cluster raises before gathering)."""
-    import torch.distributed as dist
-    world = dist.get_world_size()
+    """Multi-GPU: every rank receives every rank's records (with their headroom, and the misses, when the windows had
+    them), window by window in estimate_costs order.  The per-window record counts in one all_gather on ``device``,
+    then gather_padded of the records and of the headroom, merged by merge_rank_windows.  Every rank must have searched
+    the same windows (no fatal plan: api.cost_het_cluster raises before gathering)."""
     miss = gather_misses(merged.misses, device) if merged.misses is not None else None   # global ordinals already
     counts = torch.tensor(np.diff(merged.firsts), dtype=torch.int64, device=device)
     all_counts = _gather_rows(counts).numpy().astype(np.int64)     # [world, windows]
-    cap = max(int(all_counts.sum(axis=1).max()), 1)
-    mine = torch.zeros(cap * 2, dtype=torch.int64, device=device)
-    n_local = len(merged.records)
-    if n_local:
-        mine[:2 * n_local] = torch.from_numpy(np.ascontiguousarray(merged.records).view(np.int64).reshape(-1)).to(device)
-    got = torch.empty(world * cap * 2, dtype=torch.int64, device=device)
-    dist.all_gather_into_tensor(got, mine)
-    flat = got.cpu().numpy().view(native.RECORD_DTYPE).reshape(world, cap)
-    if merged.headroom is None:
-        rec, firsts = merge_rank_windows(all_counts, [flat[r] for r in range(world)])
-        return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts, misses=miss,
-                              misses_s=merged.misses_s)
-    # the headroom travels padded like the records, and is merged with them as one more field of each record
-    mine_h = torch.zeros(cap, dtype=torch.float64, device=device)
-    if n_local:
-        mine_h[:n_local] = torch.from_numpy(np.ascontiguousarray(merged.headroom)).to(device)
-    got_h = torch.empty(world * cap, dtype=torch.float64, device=device)
-    dist.all_gather_into_tensor(got_h, mine_h)
-    flat_h = got_h.cpu().numpy().reshape(world, cap)
-    both = np.zeros((world, cap), dtype=native.RECORD_DTYPE + [('headroom', '<f8')])
-    for f, _ in native.RECORD_DTYPE:
-        both[f] = flat[f]
-    both['headroom'] = flat_h
-    merged_both, firsts = merge_rank_windows(all_counts, [both[r] for r in range(world)])
-    rec = np.zeros(len(merged_both), dtype=native.RECORD_DTYPE)
-    for f, _ in native.RECORD_DTYPE:
-        rec[f] = merged_both[f]
-    return WindowedOutput(merged.summary, merged.best, rec, merged.bases, firsts,
-                          np.ascontiguousarray(merged_both['headroom']), merged.headroom_s, miss, merged.misses_s)
+    totals = all_counts.sum(axis=1).tolist()
+    mine = torch.from_numpy(np.ascontiguousarray(merged.records).view(np.int64).reshape(-1, 2)).to(device)
+    records = gather_padded(mine, totals).cpu().numpy().reshape(-1).view(native.RECORD_DTYPE)
+    order, firsts = merge_rank_windows(all_counts, records)
+    headroom = None
+    if merged.headroom is not None:
+        mine = torch.from_numpy(np.ascontiguousarray(merged.headroom, dtype=np.float64)).to(device)
+        headroom = gather_padded(mine, totals).cpu().numpy()[order]
+    return WindowedOutput(merged.summary, merged.best, records[order], merged.bases, firsts, headroom,
+                          merged.headroom_s, miss, merged.misses_s)
+
+
+def _rank_on_device(searcher: 'HetSearcher', buf: torch.Tensor, n: int) -> np.ndarray:
+    """Permutation (uint32) of ``sorted(records, key=cost)`` (stable) of the n device records in ``buf``, which the
+    sort reorders."""
+    dev = searcher.dp.device
+    with torch.cuda.device(dev):
+        s = torch.cuda.current_stream(dev)
+        perm = searcher.sort_records(n, native.SORT_BY_COST_STABLE, s, want_perm=True, buf=buf)
+        s.synchronize()
+        return perm.cpu().numpy().view(np.uint32)
 
 
 def make_window_ranker(searcher: 'HetSearcher', records: np.ndarray, summary: Dict):
@@ -1102,156 +1238,12 @@ def make_window_ranker(searcher: 'HetSearcher', records: np.ndarray, summary: Di
     def rank() -> np.ndarray:
         need = n * 16 + n * 4 + int(searcher.dp.lib.metis_sort_workspace_bytes(C.c_int64(n)))
         if need <= window_budget(dev, 0.0):
-            with torch.cuda.device(dev):
-                buf = torch.from_numpy(records.view(np.int64).reshape(-1)).to(dev)
-                s = torch.cuda.current_stream(dev)
-                perm = searcher.sort_records(n, native.SORT_BY_COST_STABLE, s, want_perm=True, buf=buf)
-                s.synchronize()
-                out = perm.cpu().numpy().view(np.uint32)
+            out = _rank_on_device(searcher, torch.from_numpy(records.view(np.int64).reshape(-1)).to(dev), n)
             summary['ranking'] = 'device'
             return out
         summary['ranking'] = 'host'
         return np.argsort(records['cost'], kind='stable').astype(np.uint32)
     return rank
-
-
-class WindowedCandidates:
-    """Candidates of a windowed search: only the 16 B records stay on the host.  Device groups, strategies and
-    partitions are rebuilt per request, window by window: the window's rows are regenerated on the device (row kernel)
-    and its picks replayed by metis_het_detail.  The DeviceProblem / HetSearcher of the search are reused (the arena,
-    sized for the largest window's rows, and metis_het_detail's small workspace stay allocated while the result is
-    alive); a window is reloaded whenever the arena holds something else."""
-
-    def __init__(self, records: np.ndarray, bases: np.ndarray, firsts: np.ndarray,
-                 windows: Sequence[flatten.PlanWindow], problem: flatten.FlatProblem, node_sequences: Sequence[Tuple],
-                 searcher: 'HetSearcher', headroom: Optional[np.ndarray] = None, misses: Optional[np.ndarray] = None):
-        self.records = records
-        self.misses = misses                  # MISS_HOST_DTYPE, global ordinals, reference order; else None
-        self.headroom = headroom              # float64 per record (a search with headroom), else None
-        self.device = searcher.dp.device      # where the search ran
-        self.cost = records['cost']
-        self.bases = bases
-        self.firsts = firsts
-        self.windows = list(windows)
-        self.problem = problem
-        self.node_sequences = [tuple(s) for s in node_sequences]
-        self.searcher = searcher
-
-    def __len__(self) -> int:
-        return len(self.records)
-
-    def index_of(self, ordinal: int, step: int) -> Optional[int]:
-        """(GLOBAL ordinal, step) -> position, through the window that holds the ordinal."""
-        w = int(np.searchsorted(self.bases, ordinal, side='right')) - 1
-        if w < 0 or w >= len(self.bases):
-            return None
-        rel = int(ordinal) - int(self.bases[w])
-        if rel > 0xFFFFFFFF:
-            return None
-        return _bisect_records(self.records, int(self.firsts[w]), int(self.firsts[w + 1]), rel, int(step))
-
-    def _load(self, w: int) -> DeviceProblem:
-        dp = self.searcher.dp
-        space = self.windows[w].space
-        if dp.space is not space or dp.problem is not self.problem:
-            dp.reload(self.problem, space)                    # metis_het_detail needs no more workspace than it has
-            dp.upload()
-        return dp
-
-    def tuples(self, idx) -> List[Tuple]:
-        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
-        if not len(idx):
-            return []
-        win = np.searchsorted(self.firsts, idx, side='right') - 1
-        out: List[Optional[Tuple]] = [None] * len(idx)
-        for w in np.unique(win).tolist():
-            at = np.nonzero(win == w)[0]
-            rec = self.records[idx[at]]
-            dp = self._load(w)
-            detail = self.searcher.detail_for(rec)
-            cand = Candidates(rec, detail, dp.space, self.node_sequences, rows_dev=dp.rows_device())
-            cand._BULK = 1 << 62                              # gather the rows needed, never the whole blob
-            for k, t in zip(at.tolist(), cand.tuples(np.arange(len(rec)))):
-                out[k] = t
-        return out
-
-    def _by_window(self, ordinals: np.ndarray):
-        """(window, positions into ``ordinals``, window-relative ordinals) for every window holding some of them."""
-        ordinals = np.asarray(ordinals, dtype=np.int64)
-        starts = np.asarray([w.base for w in self.windows], dtype=np.int64)
-        win = np.searchsorted(starts, ordinals, side='right') - 1
-        for w in np.unique(win).tolist():
-            at = np.nonzero(win == w)[0]
-            yield w, at, ordinals[at] - starts[w]
-
-    def plan_columns(self, ordinals: np.ndarray) -> Dict[str, np.ndarray]:
-        """Candidates.plan_columns of GLOBAL ordinals, window by window."""
-        n = len(ordinals)
-        out: Dict[str, np.ndarray] = {}
-        for w, at, rel in self._by_window(ordinals):
-            dp = self._load(w)
-            cand = Candidates(np.zeros(0, dtype=native.RECORD_DTYPE), None, dp.space, self.node_sequences,
-                              rows_dev=dp.rows_device())
-            cand._BULK = 1 << 62
-            col = cand.plan_columns(rel)
-            for k, v in col.items():
-                if k not in out:
-                    shape = (n,) + v.shape[1:] if k != 'codes' else (n, native.METIS_MAX_STAGES)
-                    out[k] = np.zeros(shape, dtype=v.dtype)
-                if k == 'codes':
-                    out[k][at, :v.shape[1]] = v
-                else:
-                    out[k][at] = v
-        return out
-
-    def trace(self, ordinals: np.ndarray) -> List[list]:
-        """verbose.decode_plan of GLOBAL ordinals, window by window."""
-        out: List[Optional[list]] = [None] * len(ordinals)
-        for w, at, rel in self._by_window(ordinals):
-            dp = self._load(w)
-            got = trace_decoded(dp.lib, dp.p_struct, dp.s_struct, self.searcher.workspace, dp.device, rel,
-                                int(dp.space.blocks['num_stage'].max()))
-            for k, t in zip(at.tolist(), got):
-                out[k] = t
-        return out
-
-    def recost(self, bandwidths: np.ndarray) -> 'Recost':
-        """Candidates.recost window by window: the detail rows of a window's records come from replaying them
-        (metis_het_detail, like tuples()), their costs go to the host ([K, N] float64)."""
-        t0 = time.perf_counter()
-        n, K = len(self.records), len(bandwidths)
-        costs = np.empty((K, n), dtype=np.float64)
-        dev = self.searcher.dp.device
-        bw = torch.from_numpy(np.ascontiguousarray(bandwidths, dtype=np.float64)).to(dev)
-        for w in range(len(self.windows)):
-            for lo in range(int(self.firsts[w]), int(self.firsts[w + 1]), _RECOST_CHUNK):
-                hi = min(int(self.firsts[w + 1]), lo + _RECOST_CHUNK)
-                rec = self.records[lo:hi]
-                dp = self._load(w)
-                with torch.cuda.device(dev):
-                    detail = torch.from_numpy(self.searcher.detail_for(rec)).to(dev)
-                    costs[:, lo:hi] = het_recost(dp.lib, dp.p_struct, dp.s_struct, self.searcher.workspace, rec, detail,
-                                                 bw, dev).cpu().numpy()
-        with torch.cuda.device(dev):
-            costs_dev = torch.from_numpy(costs).to(dev)
-        return finish_recost(self, costs_dev, costs, dev, t0)
-
-    def breakdown(self, idx, per_stage: bool = True) -> Breakdown:
-        """Cost terms and memory headroom of the candidates ``idx``, window by window like tuples()."""
-        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
-        width = max(int(self.records['num_stage'][idx].max()), 1) if len(idx) else 1
-        raw = np.zeros(len(idx), dtype=native.BREAKDOWN_DTYPE)
-        stages = np.full((len(idx), native.BD_FIELDS, width), np.nan) if per_stage else None
-        win = np.searchsorted(self.firsts, idx, side='right') - 1
-        for w in np.unique(win).tolist():
-            at = np.nonzero(win == w)[0]
-            dp = self._load(w)
-            r, st = het_breakdown(dp.lib, dp.p_struct, dp.s_struct, self.searcher.workspace, self.records[idx[at]],
-                                  dp.device, per_stage, width)
-            raw[at] = r
-            if per_stage:
-                stages[at] = st
-        return Breakdown.from_raw(raw, stages)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -1264,6 +1256,24 @@ def _gather_rows(vec: torch.Tensor) -> torch.Tensor:
     out = torch.empty(world * vec.numel(), dtype=vec.dtype, device=vec.device)
     dist.all_gather_into_tensor(out, vec)
     return out.view(world, vec.numel()).cpu()
+
+
+def _rank_counts(n: int, device) -> List[int]:
+    """``n`` of every rank (one all_gather)."""
+    return _gather_rows(torch.tensor([n], dtype=torch.int64, device=device)).reshape(-1).tolist()
+
+
+def gather_padded(rows: torch.Tensor, counts: Sequence[int]) -> torch.Tensor:
+    """Every rank's ``rows`` [counts[r], ...] (same trailing shape and dtype on every rank), concatenated in rank order
+    on ``rows.device``: ONE all_gather_into_tensor of the rows padded to the largest count."""
+    import torch.distributed as dist
+    world = dist.get_world_size()
+    cap = max(max(counts), 1)
+    pad = torch.empty((cap,) + tuple(rows.shape[1:]), dtype=rows.dtype, device=rows.device)
+    pad[:rows.shape[0]] = rows
+    got = torch.empty((world * cap,) + tuple(rows.shape[1:]), dtype=rows.dtype, device=rows.device)
+    dist.all_gather_into_tensor(got.view(-1), pad.view(-1))
+    return torch.cat([got[cap * r:cap * r + counts[r]] for r in range(world)])
 
 
 _NO_ORDINAL = 2 ** 40
@@ -1337,16 +1347,7 @@ def make_ranker(searcher: 'HetSearcher', records_dev: torch.Tensor):
     """() -> permutation of ``sorted(records, key=cost)`` (stable): the device sort on a private copy of the ordered
     records, run when a caller first asks for the ranking."""
     snap = records_dev.clone()
-    n = snap.numel() // 2
-    dev = searcher.dp.device
-
-    def rank() -> np.ndarray:
-        with torch.cuda.device(dev):
-            s = torch.cuda.current_stream(dev)
-            perm = searcher.sort_records(n, native.SORT_BY_COST_STABLE, s, want_perm=True, buf=snap)
-            s.synchronize()
-            return perm.cpu().numpy().view(np.uint32)
-    return rank
+    return lambda: _rank_on_device(searcher, snap, snap.numel() // 2)
 
 
 def check_threshold(min_headroom) -> float:
@@ -1371,10 +1372,9 @@ class HeadroomIndex:
         if not (len(headroom) == len(rank_order) == self.n):
             raise ValueError('records, headroom and rank order differ in length')
         with torch.cuda.device(self.device):
-            up = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).to(self.device)
-            self.records = up(records)
-            self.headroom = up(np.asarray(headroom, dtype=np.float64))
-            self.rank = up(np.asarray(rank_order, dtype=np.uint32))
+            self.records = upload(records, self.device)
+            self.headroom = upload(np.asarray(headroom, dtype=np.float64), self.device)
+            self.rank = upload(np.asarray(rank_order, dtype=np.uint32), self.device)
             need = int(self.lib.metis_headroom_workspace_bytes(C.c_int64(self.n)))
             self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
             self.out = torch.empty(max(self.n, 1), dtype=torch.int32, device=self.device)
@@ -1422,59 +1422,35 @@ class HeadroomIndex:
 def gather_records(out: HetSearchOutput, searcher: HetSearcher, want_rank: bool = True,
                    counts: Optional[List[int]] = None) -> HetSearchOutput:
     """Every rank receives every rank's records (+ detail rows, headroom and misses when the search had them): padded
-    tensor all_gathers over NCCL (no pickling), then the merged list is put into estimate_costs order and ranked by the
-    device sort; the misses are merged into the reference's order (gather_misses)."""
-    import torch.distributed as dist
+    tensor all_gathers over NCCL (gather_padded, no pickling), then the merged list is put into estimate_costs order and
+    ranked by the device sort, the detail rows and the headroom permuted with it; the misses are merged into the
+    reference's order (gather_misses).  ``counts``: the records of every rank, when the caller has them."""
     dev = searcher.dp.device
-    world = dist.get_world_size()
-    n_local = len(out.records)
-    if counts is None:                                        # records of every rank (global_counters has them too)
-        mine = torch.zeros(world, dtype=torch.int64, device=dev)
-        mine[dist.get_rank()] = n_local
-        dist.all_reduce(mine, op=dist.ReduceOp.SUM)
-        counts = mine.cpu().tolist()
-    cap = max(max(counts), 1)
-    stride = searcher.detail_stride
+    if counts is None:
+        counts = _rank_counts(len(out.records), dev)
     with torch.cuda.device(dev):
-        rec_pad = torch.empty(cap * 2, dtype=torch.int64, device=dev)
-        rec_pad[:2 * n_local] = out.records_dev
-        rec_g = torch.empty(world * cap * 2, dtype=torch.int64, device=dev)
-        dist.all_gather_into_tensor(rec_g, rec_pad)
-        rec_all = torch.cat([rec_g[2 * cap * r:2 * cap * r + 2 * counts[r]] for r in range(world)]).contiguous()
-        det_all = None
-        if out.detail_dev is not None:
-            det_pad = torch.empty((cap, stride), dtype=torch.uint8, device=dev)
-            det_pad[:n_local] = out.detail_dev
-            det_g = torch.empty((world * cap, stride), dtype=torch.uint8, device=dev)
-            dist.all_gather_into_tensor(det_g, det_pad)
-            det_all = torch.cat([det_g[cap * r:cap * r + counts[r]] for r in range(world)])
-        head_all = None
-        if out.headroom_dev is not None:                      # padded like the records
-            head_pad = torch.zeros(cap, dtype=torch.float64, device=dev)
-            head_pad[:n_local] = out.headroom_dev
-            head_g = torch.empty(world * cap, dtype=torch.float64, device=dev)
-            dist.all_gather_into_tensor(head_g, head_pad)
-            head_all = torch.cat([head_g[cap * r:cap * r + counts[r]] for r in range(world)])
+        rec_all = gather_padded(out.records_dev.view(-1, 2), counts).view(-1)
+        det_all = gather_padded(out.detail_dev, counts) if out.detail_dev is not None else None
+        head_all = gather_padded(out.headroom_dev, counts) if out.headroom_dev is not None else None
         n = sum(counts)
         s = torch.cuda.current_stream(dev)
         perm = searcher.sort_records(n, native.SORT_POSITION, s, want_perm=True, buf=rec_all)
-        records = searcher._to_host('records_all', rec_all[:2 * n], s).view(native.RECORD_DTYPE)
+        records = searcher._to_host('records_all', rec_all, s).view(native.RECORD_DTYPE)
         detail_dev = det_all.index_select(0, perm.long()) if det_all is not None else None
         rank_order = None
         if want_rank:
-            by_cost = rec_all[:2 * n].clone()
-            rank = searcher.sort_records(n, native.SORT_BY_COST_STABLE, s, want_perm=True, buf=by_cost)
+            rank = searcher.sort_records(n, native.SORT_BY_COST_STABLE, s, want_perm=True, buf=rec_all.clone())
             rank_order = searcher._to_host('rank_all', rank, s).view(np.uint32)
         detail = None
         if detail_dev is not None and searcher.detail_to_host:
-            detail = searcher._to_host('detail_all', detail_dev, s).reshape(n, stride)
+            detail = searcher._to_host('detail_all', detail_dev, s).reshape(n, searcher.detail_stride)
         headroom = headroom_dev = None
         if head_all is not None:
             headroom_dev = head_all.index_select(0, perm.long())
             headroom = searcher._to_host('headroom_all', headroom_dev, s).view(np.float64)
     misses = gather_misses(out.misses, dev) if out.misses is not None else None
-    return HetSearchOutput(out.summary, out.best, records, detail, out.d2h_bytes, rank_order, detail_dev,
-                           rec_all[:2 * n], headroom, headroom_dev, out.headroom_s, misses, out.misses_s)
+    return HetSearchOutput(out.summary, out.best, records, detail, out.d2h_bytes, rank_order, detail_dev, rec_all,
+                           headroom, headroom_dev, out.headroom_s, misses, out.misses_s)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -1508,21 +1484,10 @@ def closest_order(deficit: np.ndarray, device=None) -> np.ndarray:
         return np.zeros(0, dtype=np.int64)
     if n > 0xFFFFFFFF:
         raise NotImplementedError(f'ordering {n} misses: positions are 32-bit')
-    dev = _require_cuda(device)
-    lib = native.load_library()
     rows = np.zeros(n, dtype=native.MISS_DTYPE)
     rows['deficit'] = deficit
     rows['ordinal'] = np.arange(n, dtype=np.uint32)
-    with torch.cuda.device(dev):
-        buf = torch.from_numpy(rows.view(np.int64).copy()).to(dev)
-        ws = torch.empty(int(lib.metis_sort_workspace_bytes(C.c_int64(n))), dtype=torch.uint8, device=dev)
-        perm = torch.empty(n, dtype=torch.int32, device=dev)
-        s = torch.cuda.current_stream(dev)
-        rc = lib.metis_sort_records(C.c_void_p(buf.data_ptr()), C.c_int64(n), C.c_int32(native.SORT_RANKED),
-                                    C.c_void_p(perm.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_int64(ws.numel()),
-                                    C.c_void_p(s.cuda_stream))
-        native.check(rc, 'metis_sort_records')
-        return perm.cpu().numpy().view(np.uint32).astype(np.int64)
+    return sorted_positions(rows, native.SORT_RANKED, _require_cuda(device))
 
 
 def _find_attempt(items: list, call: int, attempt: int):
@@ -1619,20 +1584,12 @@ def miss_detail(candidates, misses: Misses, idx) -> MissDetail:
 
 
 def gather_misses(misses: np.ndarray, device) -> np.ndarray:
-    """Multi-rank: every rank receives every rank's misses (MISS_HOST_DTYPE, global ordinals), padded like the records
-    (one all_gather of the counts, one of the rows), merged into the reference's order."""
-    import torch.distributed as dist
-    world = dist.get_world_size()
-    counts = _gather_rows(torch.tensor([len(misses)], dtype=torch.int64, device=device)).numpy().reshape(-1)
-    cap = max(int(counts.max()), 1)
+    """Multi-rank: every rank receives every rank's misses (MISS_HOST_DTYPE, global ordinals), as int64 words through
+    gather_padded, merged into the reference's order."""
     words = MISS_HOST_DTYPE.itemsize // 8
-    mine = torch.zeros(cap * words, dtype=torch.int64, device=device)
-    if len(misses):
-        mine[:len(misses) * words] = torch.from_numpy(np.ascontiguousarray(misses).view(np.int64).reshape(-1)).to(device)
-    got = torch.empty(world * cap * words, dtype=torch.int64, device=device)
-    dist.all_gather_into_tensor(got, mine)
-    flat = got.cpu().numpy().view(MISS_HOST_DTYPE).reshape(world, cap)
-    return position_order(np.concatenate([flat[r, :int(counts[r])] for r in range(world)]))
+    mine = torch.from_numpy(np.ascontiguousarray(misses).view(np.int64).reshape(-1, words)).to(device)
+    got = gather_padded(mine, _rank_counts(len(misses), device))
+    return position_order(got.cpu().numpy().reshape(-1).view(MISS_HOST_DTYPE))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -1642,12 +1599,8 @@ def homo_costs(problem: flatten.FlatProblem, type_id: int, plans: np.ndarray, de
                ) -> Tuple[np.ndarray, np.ndarray]:
     """HomoCostEstimator.get_cost for every row (dp, pp, tp, mbs, gbs) of ``plans`` on the GPU."""
     dev = _require_cuda(device)
-    lib = native.load_library()
     with torch.cuda.device(dev):
-        tens = {k: torch.from_numpy(np.ascontiguousarray(v).view(np.uint8).reshape(-1).copy()).to(dev)
-                for k, v in problem.arrays.items()}
-        p = problem.as_struct(lambda n: tens[n].data_ptr())
-        ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=dev)
+        lib, p, _sp, ws, _keep = bind_problem(problem, dev)
         n = len(plans)
         d_plans = torch.from_numpy(np.ascontiguousarray(plans, dtype=np.int32).reshape(-1)).to(dev)
         cost = torch.zeros(max(n, 1), dtype=torch.float64, device=dev)
@@ -1666,15 +1619,11 @@ def homo_breakdown(problem: flatten.FlatProblem, type_id: int, plans: np.ndarray
     """metis_homo_breakdown for every row (dp, pp, tp, mbs, gbs) of ``plans``: (terms [n, 6], per-stage memory
     [n, largest pp] NaN-padded, status: 0 ok, 1 KeyError, 2 oom)."""
     dev = _require_cuda(device)
-    lib = native.load_library()
     plans = np.ascontiguousarray(plans, dtype=np.int32).reshape(-1, 5)
     n = len(plans)
     width = max(int(plans[:, 1].max()) if n else 1, 1)
     with torch.cuda.device(dev):
-        tens = {k: torch.from_numpy(np.ascontiguousarray(v).view(np.uint8).reshape(-1).copy()).to(dev)
-                for k, v in problem.arrays.items()}
-        p = problem.as_struct(lambda k: tens[k].data_ptr())
-        ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=dev)
+        lib, p, _sp, ws, _keep = bind_problem(problem, dev)
         d_plans = torch.from_numpy(plans.reshape(-1)).to(dev)
         terms = torch.empty((max(n, 1), 6), dtype=torch.float64, device=dev)
         mem = torch.empty((max(n, 1), width), dtype=torch.float64, device=dev)

@@ -70,7 +70,7 @@ def _trace(res, args, cluster, idx):
     """metis_het_trace + format_plan over the plans of the candidates ``idx`` (a one-search result)."""
     from metis_b200 import api, search, verbose
     cand = res.candidates
-    if not isinstance(cand, search.Candidates):
+    if cand.space is None:
         return None, 0                                    # a windowed result: no single space to trace
     ordinals = np.unique(cand.records['ordinal'][idx])
     dp = search.DeviceProblem(cand.problem, cand.space, 'cuda:0')

@@ -117,7 +117,7 @@ def run_windows(w, tmp, order, seqs, problem, space, windows, enum_ms, check):
            'host_enumeration_ms': enum_ms, 'gpu_search_ms': ms, 'plans_per_s': space.num_plans / (ms * 1e-3),
            'peak_device_bytes': int(torch.cuda.max_memory_reserved()), 'best': merged.best[:3] if merged.best else None}
     if check > 0 and space.num_plans:
-        cand = search.WindowedCandidates(merged.records, merged.bases, merged.firsts, windows, problem, seqs, searcher)
+        cand = search.window_candidates(merged, windows, problem, seqs, searcher)
         rng = random.Random(w_ndev(w) * 131 + len(w.device_types()))
         limit = row['fatal_ordinal'] if row['fatal_ordinal'] is not None else space.num_plans
         picks = sorted(rng.sample(range(limit), min(check, limit))) if limit else []
