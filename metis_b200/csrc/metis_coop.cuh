@@ -301,6 +301,50 @@ MB_HD_NOINLINE double seq_py_sum(const double *v, int n) {
     return f;
 }
 
+// First i >= lo with P[i] >= t when the index cannot tell (psub_lookup): the 32-entry window at the guess i0, then
+// the whole-table search
+template <class X>
+MB_HD_NOINLINE int psub_search(const X &x, const double *P, int N, int i0, int lo, double t) {
+    int i = x.first_ge_window(P, N, i0, lo, t);
+    if (i < 0) {
+        x.note(kPathFirstGe);
+        i = x.first_ge(P, N, t);
+        if (i < lo) i = lo;
+    }
+    return i;
+}
+
+// floor(u) for 0 <= u < 2^32, 0 for u <= 0: the bucket of u (cvt.rzi.u32.f64 clamps to the range and maps NaN to 0)
+MB_HD unsigned bucket_of(double u) {
+#ifdef __CUDA_ARCH__
+    return __double2uint_rz(u);
+#else
+    return u > 0.0 ? (unsigned)u : 0u;
+#endif
+}
+
+// First i >= lo with P[i] >= t, for t <= P[lim] and 1 <= lo <= lim (P = T.psub, non-decreasing, with its bucket
+// index IX / scale, psub_index_entry): the index's guess i = max(IX[g], lo) is checked with exact compares; when
+// P[i - 1] < t (or i == lo) and P[i + 1] >= t, the answer is i or i + 1 (i + 1 <= N: IX is capped at lim).
+// Anything else (a bucket holding several entries below t, or a guess above the answer, which monotone rounding
+// rules out) goes to psub_search.  Every branch is uniform: all lanes compute the same values.  Returns i and its
+// entry p = P[i].
+template <class X>
+MB_HD int psub_lookup(const X &x, const double *P, const uint16_t *IX, double scale, int N, int lo, double t, double &p) {
+    int i = IX[bucket_of(t * scale)];
+    if (i < lo) i = lo;
+    const double *q = P + i;
+    const double pm = q[-1], p0 = q[0], p1 = q[1];
+    if ((pm < t || i == lo) && p1 >= t) {
+        const bool up = !(p0 >= t);
+        p = up ? p1 : p0;
+        return up ? i + 1 : i;
+    }
+    i = psub_search(x, P, N, i, lo, t);
+    p = P[i];
+    return i;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // The chain evaluator.  One instance per lane (registers); `w` and `mail` are the warp's shared scratch.
 // ---------------------------------------------------------------------------------------------------------
@@ -445,25 +489,52 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         const double *dsub = T.dsub;
         const double *P = T.psub;
         // ---- prediction: uniform walk over the stages ----
+        // Stage s starting at a ends at b = min(max(first_ge(P, t) - 1, a), lim), t = perf[s] + P[a]: closed at
+        // b < lim exactly when t <= P[lim], and then the next stage starts at i = b + 1 = the first i > a with
+        // P[i] >= t, whose entry is the next P[a].
         int a = 0, first_open = -1;
-        int span = lim / last;                                // sub-layers the previous stage took: where to look first
+        const double scale = T.pidx[0];
+        if (scale > 0.0) {                                    // bucket index of psub: a lookup and a check per stage
+            const uint16_t *IX = reinterpret_cast<const uint16_t *>(T.pidx + 1);
+            const double plim = P[lim];
+            double pa = P[0];
+            int s = 0;
 #pragma unroll 1
-        for (int s = 0; s < last; ++s) {
-            int b = lim;
-            bool closed = false;
-            if (a < lim) {
-                const double t = w.perf[s] + P[a];
-                int i0 = a + span - 14;                       // a 32-entry window around the expected end
-                if (i0 < a + 1) i0 = a + 1;
-                int i = x.first_ge_window(P, N, i0, a + 1, t);
-                if (i < 0) { x.note(kPathFirstGe); i = x.first_ge(P, N, t); }
-                b = i - 1 > a ? i - 1 : a;
-                if (b >= lim) b = lim; else closed = true;
-                span = b - a;
+            for (; s < last; ++s) {
+                const double t = w.perf[s] + pa;
+                if (!(a < lim && t <= plim)) break;          // this stage and every later one stay open (NaN too)
+                const int i = psub_lookup(x, P, IX, scale, N, a + 1, t, pa);
+                if (x.leader()) { w.first[s] = (uint16_t)a; w.fe[s] = (uint16_t)((i - 1) | kBroke); }
+                a = i;
             }
-            if (x.leader()) { w.first[s] = (uint16_t)a; w.fe[s] = (uint16_t)(b | (closed ? kBroke : 0)); }
-            if (!closed && first_open < 0) first_open = s;
-            a = closed ? b + 1 : lim;
+            if (s < last) {                                   // stage s ends at lim, the later ones start there
+                first_open = s;
+                if (x.leader()) {
+#pragma unroll 1
+                    for (int u = s; u < last; ++u) { w.first[u] = (uint16_t)(u == s ? a : lim); w.fe[u] = (uint16_t)lim; }
+                }
+                a = lim;
+            }
+        } else {                                              // no index: window probes around the expected end
+            int span = lim / last;                            // sub-layers the previous stage took: where to look first
+#pragma unroll 1
+            for (int s = 0; s < last; ++s) {
+                int b = lim;
+                bool closed = false;
+                if (a < lim) {
+                    const double t = w.perf[s] + P[a];
+                    int i0 = a + span - 14;                   // a 32-entry window around the expected end
+                    if (i0 < a + 1) i0 = a + 1;
+                    int i = x.first_ge_window(P, N, i0, a + 1, t);
+                    if (i < 0) { x.note(kPathFirstGe); i = x.first_ge(P, N, t); }
+                    b = i - 1 > a ? i - 1 : a;
+                    if (b >= lim) b = lim; else closed = true;
+                    span = b - a;
+                }
+                if (x.leader()) { w.first[s] = (uint16_t)a; w.fe[s] = (uint16_t)(b | (closed ? kBroke : 0)); }
+                if (!closed && first_open < 0) first_open = s;
+                a = closed ? b + 1 : lim;
+            }
         }
         x.sync();
         x.mark(19);

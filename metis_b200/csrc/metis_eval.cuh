@@ -60,6 +60,9 @@ struct Tables {
     // to PREDICT where a stage's forward fill ends (metis_coop.cuh); every prediction is verified exactly
     const double *psub;        // [7 * num_layers + 1] (empty when norm_len < num_layers)
     const double *dsub;        // [7 * num_layers] demand of every sub-layer, dsub[j] = dlay[j / 7] (the same bits)
+    // bucket index of psub for the prediction (psub_index_entry): pidx[0] = scale (0.0: no index), then the uint16
+    // first entries IX[0 .. 7 * num_layers] of the buckets, four per double (empty with psub)
+    const double *pidx;
     // range sums (fill_range_sums below): rsum[(t * n + b) * n + a] = sum(row_t[a:b]) as CPython adds it up, n =
     // num_layers + 1; rows t: layer_memory of key t, then layer_compute of key t - num_keys, then norm_lc.  Every
     // stage of every candidate needs such a sum (memory demand, execution time, compute left after the vote); the
@@ -71,7 +74,7 @@ constexpr int kDpk = 16;
 
 // Sizes (in doubles) of the derived tables, in the order derive_tables fills them.
 struct DerivedLayout {
-    int dlay, inv_exec, ratio, dpk, pp_hidden, pp_vocab, psub, dsub, total;
+    int dlay, inv_exec, ratio, dpk, pp_hidden, pp_vocab, psub, dsub, pidx, total;
 };
 
 MB_HD DerivedLayout derived_layout(const MetisProblem &p) {
@@ -85,8 +88,59 @@ MB_HD DerivedLayout derived_layout(const MetisProblem &p) {
     d.pp_vocab = o; o += (p.num_bs + 1) * p.num_tp;
     d.psub = o; o += (p.norm_len >= p.num_layers) ? kH * p.num_layers + 1 : 0;
     d.dsub = o; o += (p.norm_len >= p.num_layers) ? kH * p.num_layers : 0;
+    d.pidx = o; o += (p.norm_len >= p.num_layers) ? 1 + (kH * p.num_layers + 1 + 3) / 4 : 0;
     d.total = o;
     return d;
+}
+
+// psub[7 r + q] (Tables::psub) from acc = norm_lc[0] + .. + norm_lc[r - 1] added up left to right, for r < norm_len
+MB_HD double psub_at(double acc, double lc_r, int q) { return acc + lc_r * ((double)q / 7.0); }
+
+// Entry k of the bucket index of psub (Tables::pidx), for the prediction walk of the forward pass (metis_coop.cuh,
+// psub_lookup).  G = N = 7 * num_layers buckets of equal width over [psub[0], psub[N]] = [0, psub[N]]; a value t
+// falls into bucket g = floor(t * scale), scale = G / psub[N].  IX[g] is the first i with psub[i] * scale >= g (the
+// product rounded like the walk's), capped at lim = N - 1 - 7: since rounding is monotone, every i with psub[i] >= t
+// has psub[i] * scale >= g, so the first such i is at least IX[g] (below lim) and at most IX[g + 1].  Entry 0 is the
+// scale, or 0.0 when psub is not non-decreasing and finite with psub[N] > 0 (a demand negative, NaN or infinite,
+// or every demand zero): the walk then searches as without an index.  Entry k >= 1 packs IX[4 (k - 1) .. + 3].
+// Each entry is computed on its own in O(num_layers) (derive_entry evaluates the derived tables entry by entry).
+MB_HD double psub_index_entry(const MetisProblem &p, const double *norm_lc, int k) {
+    const int L = p.num_layers, N = kH * L;
+    const int lim = (N - 1 - kH) > 0 ? (N - 1 - kH) : 0;
+    bool ok = N > 0;
+    double acc = 0.0;
+    for (int r = 0; r < L; ++r) {
+        ok = ok && norm_lc[r] >= 0.0 && norm_lc[r] <= 1.7976931348623157e308;
+        acc += norm_lc[r];
+    }
+    const double top = L < p.norm_len ? psub_at(acc, norm_lc[L], 0) : acc;      // psub[N]
+    const double scale = ok && top > 0.0 && top <= 1.7976931348623157e308 ? (double)N / top : 0.0;
+    if (!(scale > 0.0 && scale <= 1.7976931348623157e308)) return 0.0;
+    if (k == 0) return scale;
+    double f[kH];
+    for (int q = 0; q < kH; ++q) f[q] = (double)q / 7.0;
+    uint64_t bits = 0;
+    int r = 0;
+    acc = 0.0;                                                // psub[7 r]
+    for (int e = 0; e < 4; ++e) {
+        const double g = (double)(4 * (k - 1) + e);
+        int ix = lim;
+        while (kH * r < lim) {
+            const double nxt = acc + norm_lc[r];              // psub[7 r + 7]
+            if (nxt * scale >= g) {                           // the first entry >= g lies in psub[7 r .. 7 r + 7]
+                int q = 0;
+                while (q < kH && !((acc + norm_lc[r] * f[q]) * scale >= g)) ++q;
+                ix = kH * r + q < lim ? kH * r + q : lim;
+                break;
+            }
+            acc = nxt;
+            ++r;
+        }
+        bits |= (uint64_t)ix << (16 * e);
+    }
+    double v;
+    memcpy(&v, &bits, sizeof(v));
+    return v;
 }
 
 // One entry of the derived tables (index i of the flat array laid out by derived_layout).
@@ -101,12 +155,13 @@ MB_HD double derive_entry(const MetisProblem &p, const DerivedLayout &d, const d
         return (double)(2 * (dp - 1)) / ((double)dp * bw);
     }
     if (i < d.pp_vocab) return (double)((int64_t)(i - d.pp_hidden) * p.sequence_length * p.hidden_size) / bw;
+    if (i >= d.pidx) return psub_index_entry(p, norm_lc, i - d.pidx);
     if (i >= d.dsub) return norm_lc[(i - d.dsub) / kH] / 7.0;      // expand_lc_demand (load_balancer.py:189-193)
     if (i >= d.psub) {                                       // predictor table (see Tables::psub): whole layers + a share
         const int j = i - d.psub, r = j / kH;
         double acc = 0.0;
         for (int t = 0; t < r; ++t) acc += norm_lc[t];
-        return r < p.norm_len ? acc + norm_lc[r] * ((double)(j - r * kH) / 7.0) : acc;
+        return r < p.norm_len ? psub_at(acc, norm_lc[r], j - r * kH) : acc;
     }
     const int e = i - d.pp_vocab;
     const int mbs = e / p.num_tp, tpc = e - mbs * p.num_tp;
@@ -123,6 +178,7 @@ MB_HD void bind_derived(Tables &T, const double *base) {
     T.pp_vocab = base + d.pp_vocab;
     T.psub = base + d.psub;
     T.dsub = base + d.dsub;
+    T.pidx = base + d.pidx;
 }
 
 // One inter-stage plan (search_space/plan.py:21-29).
