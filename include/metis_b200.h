@@ -406,6 +406,78 @@ int metis_headroom_front(const MetisRecord *records, const double *headroom, con
                          uint32_t *out, uint64_t *count, void *workspace, int64_t workspace_bytes, void *stream);
 
 /*
+ * Plan queries of a finished search (metis_query.cu).  A MetisPlanFilter is a set of conditions on one candidate of
+ * the reference's estimate_costs list (cost_het_cluster.py:44-46); it selects among the candidates the search found,
+ * it does not constrain the search (the strategy chain ran unconstrained).  A candidate is admitted when
+ *   min_stages <= len(device_groups) <= max_stages, num_repartition <= max_repartition,
+ *   bit ns_idx of ns_mask and bit (index of its batches in MetisPlanSpace.batches) of div_mask are set,
+ * and, with METIS_QUERY_NEEDS_TP in flags (the tp codes of its detail row are read), every stage s has
+ *   log2(tp) <= max_tp_code; with uniform_tp, the tp of stage 0; with METIS_QUERY_BY_TYPE, log2(tp) <=
+ *   type_tp_code[d] for every device type d among the ranks [sum(groups[:s]), sum(groups[:s+1])) of the node
+ *   sequence's placement (ns_run_type / ns_run_end, model/device_group.py:22-32, 60-64).
+ * The group of an admitted candidate is the mixed radix of the digits of its num_keys key fields (first most
+ * significant); digit k is the field's value as below, in 0 .. key_range[k]-1 (outside: no group).
+ */
+#define METIS_QUERY_KEY_NS       0   /* node sequence index                                           */
+#define METIS_QUERY_KEY_STAGES   1   /* len(device_groups) - 1                                        */
+#define METIS_QUERY_KEY_BATCHES  2   /* rank of batches among the divisors of gbs, smallest first       */
+#define METIS_QUERY_KEY_MAX_TP   3   /* log2 of the largest tp of any stage (reads the detail row)     */
+#define METIS_QUERY_KEY_NREP     4   /* num_repartition - 1                                           */
+#define METIS_QUERY_MAX_KEYS     5
+#define METIS_QUERY_NEEDS_TP     1   /* flags: the conditions read the tp codes                         */
+#define METIS_QUERY_BY_TYPE      2   /* flags: type_tp_code holds a limit                               */
+#define METIS_QUERY_NO_GROUP     0xFFFFFFFFu
+
+typedef struct MetisPlanFilter {
+    int32_t min_stages, max_stages;
+    int32_t max_repartition;
+    int32_t max_tp_code;            /* 255 = no limit                                                  */
+    int32_t uniform_tp;
+    int32_t flags;                  /* METIS_QUERY_NEEDS_TP | METIS_QUERY_BY_TYPE                      */
+    uint8_t type_tp_code[METIS_MAX_TYPES];   /* per device type id; 255 = no limit                    */
+    uint32_t ns_mask[8];            /* 256 node sequences                                              */
+    uint32_t div_mask[8];           /* 256 divisors of gbs                                             */
+    int32_t num_keys;
+    int32_t key_field[METIS_QUERY_MAX_KEYS];
+    int32_t key_range[METIS_QUERY_MAX_KEYS];
+    int32_t reserved;
+} MetisPlanFilter;
+
+/*
+ * Filter and group key of n candidates, one thread each: mask[i] = 1 when candidate i is admitted and, if headroom
+ * is given, headroom[i] >= min_headroom; group[i] its group, METIS_QUERY_NO_GROUP when mask[i] == 0.
+ *   records  [device] n MetisRecord of `space` (ordinal and num_repartition are read)
+ *   detail   [device] n rows of detail_stride bytes aligned with records (the search's layout), or NULL when flags has
+ *            no METIS_QUERY_NEEDS_TP and no key is METIS_QUERY_KEY_MAX_TP
+ *   headroom [device] n doubles aligned with records, or NULL;  mask [device] n bytes;  group [device] n uint32 or NULL
+ * Reads only the problem's ns_run_type / ns_run_end and the space: no workspace, no table packing.
+ */
+int metis_query_mark(const MetisProblem *problem, const MetisPlanSpace *space, const MetisPlanFilter *filter,
+                     const MetisRecord *records, int64_t n, const uint8_t *detail, int32_t detail_stride,
+                     const double *headroom, double min_headroom, uint8_t *mask, uint32_t *group, void *stream);
+
+/*
+ * Best candidate of every group: over the n candidates with group[i] != METIS_QUERY_NO_GROUP (group[i] <
+ * num_groups <= 2^24), count[g] members, cost[g] the lowest cost and first[g] the lowest position i of a member with
+ * that cost (-0.0 and +0.0 are one cost), present[g] = count[g] > 0.  Exact whatever the order of the atomics.
+ *   records [device] n MetisRecord (the cost is read);  group [device] n uint32
+ *   count [device] num_groups uint64;  cost [device] num_groups doubles (+inf without members);
+ *   first [device] num_groups int64 (-1 without members);  present [device] num_groups bytes
+ */
+int metis_query_groups(const MetisRecord *records, const uint32_t *group, int64_t n, int64_t num_groups,
+                       uint64_t *count, double *cost, int64_t *first, uint8_t *present, void *stream);
+
+/*
+ * Stable compaction of a byte mask (metis_select.cu, the two-level pass of metis_headroom_select): the first k
+ * entries i of 0..n-1 whose mask[order[i]] != 0 (order = NULL: the identity), in that order, written as order[i] (i)
+ * to out [device, k uint32]; *count [host] = how many qualify.  With order = the rank permutation of
+ * metis_sort_records(METIS_SORT_BY_COST_STABLE) this is a ranked selection under a filter.
+ *   workspace [device] metis_headroom_workspace_bytes(n) bytes
+ */
+int metis_mask_select(const uint8_t *mask, const uint32_t *order, int64_t n, int64_t k, uint32_t *out, uint64_t *count,
+                      void *workspace, int64_t workspace_bytes, void *stream);
+
+/*
  * Host-side enumeration of gen_dgroups_for_stages_with_variance (search_space/device_group.py:93-107)
  * in reference order.  Writes log2 codes, num_stages bytes per row, into out (host memory) and
  * returns the number of rows, or METIS_E_CAPACITY if capacity_rows is too small (call with

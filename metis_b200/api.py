@@ -218,10 +218,24 @@ class HetSearchResult(Sequence):
         """fp64 cost of every candidate, estimate_costs order (no tuples built)."""
         return self.candidates.cost
 
-    def ranked(self, k: Optional[int] = None, min_headroom: Optional[float] = None) -> List[Tuple]:
+    def ranked(self, k: Optional[int] = None, min_headroom: Optional[float] = None, where=None) -> List[Tuple]:
         """The first ``k`` (default: all) entries of ``sorted(result, key=lambda kv: kv[6])``.  With ``min_headroom``
         (MB, finite; needs ``headroom=True``): the first ``k`` of those whose headroom is at least that, in ranked
-        order (metis_headroom_select on the GPU); ``k`` must then be >= 0 (a count, not a slice bound)."""
+        order (metis_headroom_select on the GPU); ``k`` must then be >= 0 (a count, not a slice bound).
+
+        ``where`` (a search.PlanFilter): only the candidates it admits, ``[t for t in sorted(result, key=cost) if
+        where.admits(t)]``, then the ``min_headroom`` condition, then the first ``k`` (metis_query_mark and
+        metis_mask_select on the GPU).  The filter selects among the candidates this search found; it does not
+        constrain the search."""
+        if where is not None:
+            from . import search
+            if min_headroom is not None and k is not None and int(k) < 0:
+                raise ValueError(f'k must be >= 0 with min_headroom, not {k}')
+            mask, _group = self._mark(where, min_headroom)
+            n = len(self)
+            sliced = k is None or int(k) < 0
+            pos, _total = search.mask_select(mask, n, self._rank_device(), n if sliced else int(k))
+            return self.candidates.tuples(pos[:k] if sliced and k is not None else pos)
         if min_headroom is not None:
             from . import search
             x = search.check_threshold(min_headroom)
@@ -234,6 +248,90 @@ class HetSearchResult(Sequence):
         if k is not None:
             order = order[:k]
         return self.candidates.tuples(order)
+
+    def count(self, where=None, min_headroom: Optional[float] = None) -> int:
+        """How many candidates ``where`` (a search.PlanFilter, default: all) admits with headroom >= ``min_headroom``
+        (needs ``headroom=True``), counted on the GPU."""
+        if where is None and min_headroom is None:
+            return len(self)
+        from . import search
+        mask, _group = self._mark(where, min_headroom)
+        return search.mask_select(mask, len(self), None, 0)[1]
+
+    def best_by(self, keys, where=None, min_headroom: Optional[float] = None):
+        """The best admitted candidate per key value: ``keys`` is a subset of ('node_sequence', 'num_stage', 'batches',
+        'max_tp', 'num_repartition') ('max_tp': the largest tp of any stage).  For every value of the keys that some
+        candidate admitted by ``where`` (with headroom >= ``min_headroom``) has, a search.Groups row holds the values,
+        the count and the first such candidate of sorted(result, key=cost) - lowest cost, then lowest estimate_costs
+        position - as its position and cost (``.tuples()`` builds them), in ascending key order.  Computed on the GPU
+        over a dense table of groups, at most 2^24 (metis_query_groups)."""
+        from . import search
+        keys = search.check_keys(keys)
+        cand = self.candidates
+        n = len(cand.records)
+        ranges = {'node_sequence': len(cand.node_sequences),
+                  'num_stage': max(int(cand.records['num_stage'].max()), 1) if n else 1,
+                  'batches': len(self._batches()), 'max_tp': int(cand.problem.scalars['num_tp']),
+                  'num_repartition': 3}
+        num_groups = int(np.prod([ranges[k] for k in keys], dtype=np.float64))
+        if num_groups > 1 << 24:
+            raise ValueError(f'best_by{keys}: {num_groups} groups, more than 2^24')
+        mask, group = self._mark(where, min_headroom, keys, [ranges[k] for k in keys])
+        admitted = search.mask_select(mask, n, None, 0)[1]
+        ids, count, _cost, first = search.group_best(cand.records_device(), group, n, num_groups)
+        if int(count.sum()) != admitted:
+            raise native.MetisNativeError(f'best_by{keys}: {admitted - int(count.sum())} admitted candidates outside '
+                                          f'the key ranges {ranges}')
+        batches = self._batches()
+        digits = []
+        rest = ids.copy()
+        for k in reversed(keys):
+            digits.append(rest % ranges[k])
+            rest //= ranges[k]
+        digits = digits[::-1]
+        decode = {'node_sequence': lambda d: cand.node_sequences[d], 'num_stage': lambda d: d + 1,
+                  'batches': lambda d: int(batches[len(batches) - 1 - d]), 'max_tp': lambda d: 1 << d,
+                  'num_repartition': lambda d: d + 1}
+        values = [tuple(decode[k](int(digits[j][g])) for j, k in enumerate(keys)) for g in range(len(ids))]
+        order = sorted(range(len(values)), key=lambda g: tuple(search._names(v) if k == 'node_sequence' else v
+                                                               for k, v in zip(keys, values[g])))
+        pos = first[order].astype(np.int64)
+        return search.Groups(cand, keys, [values[g] for g in order], count[order].astype(np.int64), pos,
+                             np.array(self.costs[pos]))
+
+    def _batches(self) -> np.ndarray:
+        """The divisors of gbs every plan space of the result enumerates (MetisPlanSpace.batches)."""
+        spaces = [s.space for s in self.candidates.segments]
+        b = spaces[0].batches
+        if any(not np.array_equal(s.batches, b) for s in spaces[1:]):
+            raise NotImplementedError('the windows of this result enumerate different batches')
+        return b
+
+    def _mark(self, where, min_headroom, keys=(), key_ranges=()):
+        """metis_query_mark of ``where`` (and the headroom threshold) on every candidate: (mask, group) on the device."""
+        from . import search
+        where = search.PlanFilter() if where is None else where
+        if not isinstance(where, search.PlanFilter):
+            raise TypeError(f'where must be a search.PlanFilter, not {type(where).__name__}')
+        cand = self.candidates
+        flt = where.to_struct(cand.problem.type_names, cand.node_sequences, self._batches())
+        flt.num_keys = len(keys)
+        for j, k in enumerate(keys):
+            flt.key_field[j] = search.QUERY_KEYS.index(k)
+            flt.key_range[j] = key_ranges[j]
+        headroom, x = None, 0.0
+        if min_headroom is not None:
+            x = search.check_threshold(min_headroom)
+            headroom = self._index().headroom
+        return cand.query(flt, where.reads_strategies or 'max_tp' in keys, headroom, x, groups=bool(keys))
+
+    def _rank_device(self):
+        """The rank permutation on the device (uploaded once)."""
+        if getattr(self, '_rank_dev', None) is None:
+            from . import search
+            self._rank_dev = search.upload(np.ascontiguousarray(self._rank(), dtype=np.uint32),
+                                           search._require_cuda(self.candidates.device))
+        return self._rank_dev
 
     def _rank(self) -> np.ndarray:
         if self.rank_order is None:

@@ -84,6 +84,14 @@ struct LastOfRunItems {              // record t (of *m) whose successor has ano
     __device__ uint32_t value(long long t) const { return rank[recs[t]]; }
 };
 
+struct MaskItems {                   // entries whose order[i] (i without an order) is marked -> order[i]
+    const uint8_t *mask;
+    const uint32_t *order;
+    __device__ uint32_t at(long long i) const { return order ? __ldg(&order[i]) : (uint32_t)i; }
+    __device__ bool flag(long long i) const { return __ldg(&mask[at(i)]) != 0; }
+    __device__ uint32_t value(long long i) const { return at(i); }
+};
+
 template <class F>
 __global__ void __launch_bounds__(kSelThreads) count_kernel(F f, long long n, unsigned long long *tile_count) {
     const long long first = blockIdx.x * kTile + (long long)threadIdx.x * kItems;
@@ -273,6 +281,18 @@ int metis_headroom_front(const MetisRecord *records, const double *headroom, con
     rc = compact(RecordItems{w.flags}, n, w, w.totals, w.recs, n, stream);
     if (rc) return rc;
     rc = compact(LastOfRunItems{records, rank, w.recs, w.totals}, n, w, w.totals + 1, out, n, stream);
+    return rc ? rc : send_count(w.totals + 1, count, stream);
+}
+
+int metis_mask_select(const uint8_t *mask, const uint32_t *order, int64_t n, int64_t k, uint32_t *out, uint64_t *count,
+                      void *workspace, int64_t workspace_bytes, void *stream_) {
+    if (n < 0 || n > 0xFFFFFFFFLL) return fail_arg("metis_mask_select: n out of range (0 .. 2^32 - 1)");
+    if ((n > 0 && !mask) || !count || !workspace) return fail_arg("metis_mask_select: NULL argument");
+    if (k < 0 || (k > 0 && !out)) return fail_arg("metis_mask_select: bad k / out");
+    if (workspace_bytes < metis_headroom_workspace_bytes(n)) return METIS_E_CAPACITY;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const SelectWorkspace w = carve_select(workspace, n);
+    const int rc = compact(MaskItems{mask, order}, n, w, w.totals + 1, out, k < n ? k : n, stream);
     return rc ? rc : send_count(w.totals + 1, count, stream);
 }
 

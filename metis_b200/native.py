@@ -73,6 +73,18 @@ class MetisListing(C.Structure):
                 ('reserved', C.c_int32)]
 
 
+class MetisPlanFilter(C.Structure):
+    _fields_ = [('min_stages', C.c_int32), ('max_stages', C.c_int32), ('max_repartition', C.c_int32),
+                ('max_tp_code', C.c_int32), ('uniform_tp', C.c_int32), ('flags', C.c_int32),
+                ('type_tp_code', C.c_uint8 * METIS_MAX_TYPES), ('ns_mask', C.c_uint32 * 8), ('div_mask', C.c_uint32 * 8),
+                ('num_keys', C.c_int32), ('key_field', C.c_int32 * 5), ('key_range', C.c_int32 * 5),
+                ('reserved', C.c_int32)]
+
+
+QUERY_KEYS = ('node_sequence', 'num_stage', 'batches', 'max_tp', 'num_repartition')   # METIS_QUERY_KEY_* order
+QUERY_NEEDS_TP, QUERY_BY_TYPE = 1, 2
+QUERY_NO_GROUP = 0xFFFFFFFF
+
 assert C.sizeof(MetisRecord) == 16 and C.sizeof(MetisPlanBlock) == 32
 
 # numpy dtype twins of the C structs
@@ -95,7 +107,7 @@ SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 
            'metis_enum_compositions', 'metis_generate_rows', 'metis_list_workspace_bytes', 'metis_list_stages',
            'metis_list_window', 'metis_het_search_headroom', 'metis_headroom_workspace_bytes', 'metis_headroom_select',
            'metis_headroom_front', 'metis_het_search_outputs', 'metis_het_recost', 'metis_recost_regret_workspace_bytes',
-           'metis_recost_regret']
+           'metis_recost_regret', 'metis_query_mark', 'metis_query_groups', 'metis_mask_select']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -159,6 +171,16 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_recost_regret.restype = C.c_int
     lib.metis_recost_regret.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_void_p]
+    lib.metis_query_mark.restype = C.c_int
+    lib.metis_query_mark.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisPlanFilter),
+                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_void_p,
+                                     C.c_void_p, C.c_void_p]
+    lib.metis_query_groups.restype = C.c_int
+    lib.metis_query_groups.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]
+    lib.metis_mask_select.restype = C.c_int
+    lib.metis_mask_select.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int64, C.c_void_p]
     lib.metis_homo_breakdown.restype = C.c_int
     lib.metis_homo_breakdown.argtypes = [C.POINTER(MetisProblem), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
                                          C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

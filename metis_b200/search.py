@@ -101,6 +101,7 @@ class DeviceProblem:
         self._off: Dict[str, Tuple[int, int]] = {}           # name -> (offset, capacity)
         self._used: Dict[str, int] = {}
         self._reserve: Dict[str, int] = {}
+        self._uploaded = None       # event after the last upload's copy: until then the copy may still read _host
         for w in reserve:
             for name, n in w.arena_sizes().items():
                 self._reserve[name] = max(self._reserve.get(name, 0), n)
@@ -147,6 +148,7 @@ class DeviceProblem:
         """Stage another problem / space (host side only; call upload()).  Tables that already live in the staging
         arena (``build_plan_space(rows_out=staging('rows'))``) are not copied again."""
         flat = self._arrays(problem, space)
+        self._wait_upload()
         if not self.fits(problem, space):
             keep = {n: flat[n].copy() for n in _ARENA_ORDER}     # a view into the old arena must survive the swap
             self._allocate(keep, space, 0)
@@ -168,8 +170,16 @@ class DeviceProblem:
 
     def staging(self, name: str) -> np.ndarray:
         """The pinned host region of one table (numpy view, full capacity): fill it in place, then upload()."""
+        self._wait_upload()
         off, cap = self._off[name]
         return self._host.numpy()[off:off + cap]
+
+    def _wait_upload(self) -> None:
+        """Block until the last upload's copy has read the pinned staging arena: the copy is asynchronous, so a host
+        write into the arena (reload, staging) before it ran would reach the device as the next problem's tables."""
+        if self._uploaded is not None:
+            self._uploaded.synchronize()
+            self._uploaded = None
 
     def restage_space(self, space: flatten.FlatPlanSpace) -> None:
         """Put a freshly enumerated space into the staging arena (same problem)."""
@@ -180,6 +190,8 @@ class DeviceProblem:
         n = self.h2d_bytes
         with torch.cuda.device(self.device), torch.cuda.stream(stream or torch.cuda.current_stream(self.device)):
             self._dev[:n].copy_(self._host[:n], non_blocking=True)
+            self._uploaded = torch.cuda.Event()
+            self._uploaded.record()
             if self.device_rows:                              # SURVEY.md 8(f)-1: the GPU writes the rows itself
                 base = self._dev.data_ptr()
                 s = torch.cuda.current_stream(self.device)
@@ -652,6 +664,270 @@ class Candidates:
         best, regret = recost_regret(costs_dev)
         t2 = time.perf_counter()
         return Recost(self, costs, best, regret, dev, {'recost_s': t1 - t0, 'regret_s': t2 - t1})
+
+    def records_device(self) -> torch.Tensor:
+        """The records (estimate_costs order) on the device, uploaded on first use: what the group passes read."""
+        if getattr(self, '_records_dev', None) is None:
+            self._records_dev = upload(self.records, _require_cuda(self.device))
+        return self._records_dev
+
+    def query(self, flt: native.MetisPlanFilter, reads_tp: bool, headroom: Optional[torch.Tensor] = None,
+              min_headroom: float = 0.0, groups: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """The filter ``flt`` on every candidate (metis_query_mark), segment by segment, _RECOST_CHUNK records per
+        launch: (mask, uint8 [N] on the device; group, int32 [N] (uint32 bits), when ``groups``).  The detail rows are
+        read only when ``reads_tp`` (a window replays them then); ``headroom`` (device, aligned with the records) ANDs
+        in headroom >= min_headroom.  Nothing comes to the host."""
+        dev = _require_cuda(self.device)
+        n = len(self.records)
+        with torch.cuda.device(dev):
+            recs = self.records_device()
+            mask = torch.zeros(max(n, 1), dtype=torch.uint8, device=dev)
+            group = torch.empty(max(n, 1), dtype=torch.int32, device=dev) if groups else None
+            s = torch.cuda.current_stream(dev)
+            for seg in self.segments:
+                if seg.first == seg.end:                      # nothing to mark: a window is not reloaded for it
+                    continue
+                lib, p, sp, _ws, _dev, _keep = seg.bind()
+                for lo in range(seg.first, seg.end, _RECOST_CHUNK):
+                    hi = min(seg.end, lo + _RECOST_CHUNK)
+                    detail = seg.detail_device(lo - seg.first, hi - seg.first, self.records[lo:hi], dev) \
+                        if reads_tp else None
+                    rc = lib.metis_query_mark(
+                        C.byref(p), C.byref(sp), C.byref(flt), C.c_void_p(recs.data_ptr() + 16 * lo), C.c_int64(hi - lo),
+                        C.c_void_p(detail.data_ptr() if detail is not None else 0),
+                        C.c_int32(detail.shape[1] if detail is not None else 0),
+                        C.c_void_p(headroom.data_ptr() + 8 * lo if headroom is not None else 0), C.c_double(min_headroom),
+                        C.c_void_p(mask.data_ptr() + lo), C.c_void_p(group.data_ptr() + 4 * lo if groups else 0),
+                        C.c_void_p(s.cuda_stream))
+                    native.check(rc, 'metis_query_mark')
+        return mask, group
+
+
+def mask_select(mask: torch.Tensor, n: int, order: Optional[torch.Tensor], k: int) -> Tuple[np.ndarray, int]:
+    """metis_mask_select: (the first ``k`` entries i whose mask[order[i]] (mask[i] without ``order``) is set, as
+    order[i] (i), int64 on the host; how many are set in all)."""
+    lib = native.load_library()
+    dev = mask.device
+    k = max(0, min(int(k), n))
+    with torch.cuda.device(dev):
+        ws = torch.empty(int(lib.metis_headroom_workspace_bytes(C.c_int64(n))), dtype=torch.uint8, device=dev)
+        out = torch.empty(max(k, 1), dtype=torch.int32, device=dev)
+        count = torch.zeros(1, dtype=torch.int64).pin_memory()
+        s = torch.cuda.current_stream(dev)
+        rc = lib.metis_mask_select(C.c_void_p(mask.data_ptr()), C.c_void_p(order.data_ptr() if order is not None else 0),
+                                   C.c_int64(n), C.c_int64(k), C.c_void_p(out.data_ptr()), C.c_void_p(count.data_ptr()),
+                                   C.c_void_p(ws.data_ptr()), C.c_int64(ws.numel()), C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_mask_select')
+        s.synchronize()
+        total = int(count[0])
+        return out[:min(k, total)].cpu().numpy().view(np.uint32).astype(np.int64), total
+
+
+def group_best(records: torch.Tensor, group: torch.Tensor, n: int, num_groups: int
+               ) -> Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """metis_query_groups, then the groups with members compacted on the device (metis_mask_select): (group ids,
+    counts, lowest costs, first positions of that cost), host arrays, by ascending group id."""
+    lib = native.load_library()
+    dev = records.device
+    with torch.cuda.device(dev):
+        count = torch.empty(num_groups, dtype=torch.int64, device=dev)
+        cost = torch.empty(num_groups, dtype=torch.float64, device=dev)
+        first = torch.empty(num_groups, dtype=torch.int64, device=dev)
+        present = torch.empty(num_groups, dtype=torch.uint8, device=dev)
+        s = torch.cuda.current_stream(dev)
+        rc = lib.metis_query_groups(C.c_void_p(records.data_ptr()), C.c_void_p(group.data_ptr()), C.c_int64(n),
+                                    C.c_int64(num_groups), C.c_void_p(count.data_ptr()), C.c_void_p(cost.data_ptr()),
+                                    C.c_void_p(first.data_ptr()), C.c_void_p(present.data_ptr()), C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_query_groups')
+        ids, _m = mask_select(present, num_groups, None, num_groups)
+        at = torch.from_numpy(ids).to(dev)
+        return (ids, count.index_select(0, at).cpu().numpy(), cost.index_select(0, at).cpu().numpy(),
+                first.index_select(0, at).cpu().numpy())
+
+
+# ---------------------------------------------------------------------------------------------
+# plan queries: filters on the candidates and the best candidate per key (metis_query.cu)
+# ---------------------------------------------------------------------------------------------
+QUERY_KEYS = native.QUERY_KEYS
+_NO_LIMIT = 255
+_MAX_GROUPS = 1 << 24
+
+
+def _is_int(v) -> bool:
+    return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+
+
+def _tp_code(field: str, t) -> int:
+    if not _is_int(t) or t < 1 or t & (t - 1):
+        raise ValueError(f'{field} must be a positive power of two, not {t!r}')
+    return min(int(t).bit_length() - 1, _NO_LIMIT - 1)
+
+
+def _clamp(v: Optional[int], default: int) -> int:
+    return default if v is None else max(-1, min(int(v), 1 << 30))
+
+
+def _names(seq) -> Tuple[str, ...]:
+    return tuple(flatten._type_name(x) for x in seq)
+
+
+@dataclass(frozen=True)
+class PlanFilter:
+    """Conditions on one of the reference's candidates, the 7-tuple (node_sequence, device_groups, strategies, batches,
+    layer_partition, num_repartition, cost); a field left at None (False) sets no condition.  A filter selects among
+    the candidates a search found: it is not a search that forbids strategies.  The strategy chain ran unconstrained,
+    so a search constrained the same way could find plans that are not in the list.
+
+    ``admits(t, placement)`` is the definition; the GPU (metis_query_mark) computes the same on every candidate."""
+    min_stages: Optional[int] = None              # min_stages <= len(device_groups)
+    max_stages: Optional[int] = None              # len(device_groups) <= max_stages
+    node_sequences: Optional[Sequence[Sequence]] = None   # node_sequence is one of these (by device-type name)
+    batches: Optional[Sequence[int]] = None       # batches is one of these
+    max_tp: Optional[int] = None                  # every stage's tp <= max_tp
+    max_tp_by_type: Optional[Dict[str, int]] = None   # every stage that holds a device of type d has tp <= [d]
+    uniform_tp: bool = False                      # every stage has the same tp
+    max_repartition: Optional[int] = None         # num_repartition <= max_repartition
+
+    @property
+    def reads_strategies(self) -> bool:
+        """Whether the conditions read the strategies (then a query reads the detail rows)."""
+        return self.max_tp is not None or bool(self.max_tp_by_type) or bool(self.uniform_tp)
+
+    def admits(self, t: Tuple, placement=None) -> bool:
+        """Does candidate ``t`` pass?  ``placement``: the reference's rank_device_map of t's node sequence (rank ->
+        device type name, model/device_group.py:22-32), needed with ``max_tp_by_type``: stage s holds the ranks
+        [sum(groups[:s]), sum(groups[:s+1]))."""
+        ns, groups, strategies, batches, _part, nrep, _cost = t
+        S = len(groups)
+        if self.min_stages is not None and S < self.min_stages:
+            return False
+        if self.max_stages is not None and S > self.max_stages:
+            return False
+        if self.node_sequences is not None and _names(ns) not in {_names(q) for q in self.node_sequences}:
+            return False
+        if self.batches is not None and batches not in set(self.batches):
+            return False
+        if self.max_repartition is not None and nrep > self.max_repartition:
+            return False
+        tps = [tp for _dp, tp in strategies]
+        if self.max_tp is not None and any(tp > self.max_tp for tp in tps):
+            return False
+        if self.uniform_tp and len(set(tps)) > 1:
+            return False
+        if self.max_tp_by_type:
+            lo = 0
+            for g, tp in zip(groups, tps):
+                for r in range(lo, lo + g):
+                    limit = self.max_tp_by_type.get(placement[r])
+                    if limit is not None and tp > limit:
+                        return False
+                lo += g
+        return True
+
+    def check(self, type_names: Sequence[str]) -> None:
+        """ValueError naming the field when a field is not valid for a cluster of the device types ``type_names``."""
+        for field in ('min_stages', 'max_stages', 'max_repartition'):
+            v = getattr(self, field)
+            if v is not None and not _is_int(v):
+                raise ValueError(f'{field} must be an int, not {v!r}')
+        if self.min_stages is not None and self.max_stages is not None and self.min_stages > self.max_stages:
+            raise ValueError(f'min_stages ({self.min_stages}) > max_stages ({self.max_stages})')
+        if self.max_tp is not None:
+            _tp_code('max_tp', self.max_tp)
+        for name, t in (self.max_tp_by_type or {}).items():
+            if name not in type_names:
+                raise ValueError(f'max_tp_by_type: unknown device type {name!r} (the cluster has {list(type_names)})')
+            _tp_code(f'max_tp_by_type[{name!r}]', t)
+        for q in self.node_sequences if self.node_sequences is not None else ():
+            if isinstance(q, str) or sorted(_names(q)) != sorted(type_names):
+                raise ValueError(f'node_sequences: {q!r} is not a permutation of the cluster device types '
+                                 f'{list(type_names)}')
+        for b in self.batches if self.batches is not None else ():
+            if not _is_int(b):
+                raise ValueError(f'batches must hold ints, not {b!r}')
+
+    def to_struct(self, type_names: Sequence[str], node_sequences: Sequence[Tuple], batches: np.ndarray
+                  ) -> native.MetisPlanFilter:
+        """The MetisPlanFilter of this filter for candidates of ``node_sequences`` and the divisors ``batches``."""
+        self.check(type_names)
+        f = native.MetisPlanFilter()
+        # stage counts and num_repartition are small: clamping keeps every bound's meaning inside int32
+        f.min_stages = _clamp(self.min_stages, 0)
+        f.max_stages = _clamp(self.max_stages, 1 << 30)
+        f.max_repartition = _clamp(self.max_repartition, 1 << 30)
+        f.max_tp_code = _tp_code('max_tp', self.max_tp) if self.max_tp is not None else _NO_LIMIT
+        f.uniform_tp = int(bool(self.uniform_tp))
+        for k in range(native.METIS_MAX_TYPES):
+            f.type_tp_code[k] = _NO_LIMIT
+        for name, t in (self.max_tp_by_type or {}).items():
+            f.type_tp_code[list(type_names).index(name)] = _tp_code('max_tp_by_type', t)
+        f.flags = (native.QUERY_NEEDS_TP if self.reads_strategies else 0) | \
+            (native.QUERY_BY_TYPE if self.max_tp_by_type else 0)
+        want = {_names(q) for q in self.node_sequences} if self.node_sequences is not None else None
+        for i, q in enumerate(node_sequences):
+            if want is None or _names(q) in want:
+                f.ns_mask[i >> 5] |= 1 << (i & 31)
+        want_b = {int(b) for b in self.batches} if self.batches is not None else None
+        if len(batches) > 256:
+            raise NotImplementedError(f'{len(batches)} divisors of gbs: a filter addresses 256')
+        for i, b in enumerate(batches.tolist()):
+            if want_b is None or int(b) in want_b:
+                f.div_mask[i >> 5] |= 1 << (i & 31)
+        return f
+
+
+def query_key(t: Tuple, keys: Sequence[str]) -> Tuple:
+    """The values of ``keys`` (of QUERY_KEYS) of candidate ``t``; 'max_tp' is the largest tp of any stage."""
+    val = {'node_sequence': lambda: t[0], 'num_stage': lambda: len(t[1]), 'batches': lambda: t[3],
+           'max_tp': lambda: max(tp for _dp, tp in t[2]), 'num_repartition': lambda: t[5]}
+    return tuple(val[k]() for k in keys)
+
+
+def check_keys(keys) -> Tuple[str, ...]:
+    if isinstance(keys, str):
+        keys = (keys,)
+    keys = tuple(keys)
+    if not keys:
+        raise ValueError('keys: at least one key')
+    for k in keys:
+        if k not in QUERY_KEYS:
+            raise ValueError(f'keys: unknown key {k!r} (choose from {QUERY_KEYS})')
+    if len(set(keys)) != len(keys):
+        raise ValueError(f'keys: {keys} repeats a key')
+    return keys
+
+
+def rank_device_map(problem: flatten.FlatProblem, ns_idx: int) -> List[str]:
+    """The device type name of every rank under node sequence ``ns_idx`` (the reference's rank_device_map,
+    model/device_group.py:22-32), from the problem's ns_run_type / ns_run_end."""
+    a = problem.arrays
+    out: List[str] = []
+    for typ, end in zip(a['ns_run_type'][ns_idx].tolist(), a['ns_run_end'][ns_idx].tolist()):
+        out += [problem.type_names[typ]] * (end - len(out))
+    return out
+
+
+class Groups:
+    """The best candidate of every key value (HetSearchResult.best_by): for each value of ``keys`` that some admitted
+    candidate has, in ascending key order (node sequences by their type names), ``values[g]`` (the key values),
+    ``count[g]`` (admitted candidates with them), ``position[g]`` (estimate_costs position of the first of them in
+    sorted(result, key=cost), i.e. lowest cost, then lowest position) and ``cost[g]``."""
+
+    def __init__(self, candidates, keys: Tuple[str, ...], values: List[Tuple], count: np.ndarray, position: np.ndarray,
+                 cost: np.ndarray):
+        self.candidates = candidates
+        self.keys = keys
+        self.values = values
+        self.count = count
+        self.position = position
+        self.cost = cost
+
+    def __len__(self) -> int:
+        return len(self.values)
+
+    def tuples(self) -> List[Tuple]:
+        """The reference's 7-tuple of each group's best candidate."""
+        return self.candidates.tuples(self.position)
 
 
 _BULK = 4096           # rows a one-search result gathers on the device per request; more are fetched whole, once
