@@ -44,27 +44,34 @@ static inline BlobLayout make_layout(const MetisProblem &p) {
     return l;
 }
 
-// `base`: the staged tables (shared or global memory); `gblob`: the blob in global memory when its range-sum tables
-// were filled for this launch (search kernels), else nullptr
-__device__ __forceinline__ Tables make_tables(const MetisProblem &p, const BlobLayout &l, const uint8_t *base,
-                                              const uint8_t *gblob = nullptr) {
-    Tables T;
+// `base`: the staged tables (a plain pointer to global memory, or the shared-memory address of the staged copy);
+// `gblob`: the blob in global memory when its range-sum tables were filled for this launch (search kernels), else
+// nullptr
+template <class Space>
+__device__ __forceinline__ TablesOf<Space> bind_tables(const MetisProblem &p, const BlobLayout &l,
+                                                       typename Space::template ptr<uint8_t> base, const uint8_t *gblob) {
+    TablesOf<Space> T;
     T.p = p;
     T.rsum = gblob ? reinterpret_cast<const double *>(gblob + l.rsum) : nullptr;
-    T.key_index = reinterpret_cast<const int16_t *>(base + l.key);
-    T.lc = reinterpret_cast<const double *>(base + l.lc);
-    T.mem = reinterpret_cast<const double *>(base + l.mem);
-    T.exec_full = reinterpret_cast<const double *>(base + l.exec_full);
-    T.fb_sync = reinterpret_cast<const double *>(base + l.fb);
-    T.norm_lc = reinterpret_cast<const double *>(base + l.norm);
-    bind_derived(T, reinterpret_cast<const double *>(base + l.derived));
-    T.type_memory = reinterpret_cast<const double *>(base + l.tmem);
-    T.bw_first = reinterpret_cast<const double *>(base + l.bwf);
-    T.bw_min = reinterpret_cast<const double *>(base + l.bwm);
+    T.key_index = tab_cast<int16_t>(base + l.key);
+    T.lc = tab_cast<double>(base + l.lc);
+    T.mem = tab_cast<double>(base + l.mem);
+    T.exec_full = tab_cast<double>(base + l.exec_full);
+    T.fb_sync = tab_cast<double>(base + l.fb);
+    T.norm_lc = tab_cast<double>(base + l.norm);
+    bind_derived(T, tab_cast<double>(base + l.derived));
+    T.type_memory = tab_cast<double>(base + l.tmem);
+    T.bw_first = tab_cast<double>(base + l.bwf);
+    T.bw_min = tab_cast<double>(base + l.bwm);
     T.run_type = base + l.runt;
-    T.run_end = reinterpret_cast<const int32_t *>(base + l.rune);
-    T.q10_end = reinterpret_cast<const int32_t *>(base + l.q10e);
+    T.run_end = tab_cast<int32_t>(base + l.rune);
+    T.q10_end = tab_cast<int32_t>(base + l.q10e);
     return T;
+}
+
+__device__ __forceinline__ Tables make_tables(const MetisProblem &p, const BlobLayout &l, const uint8_t *base,
+                                              const uint8_t *gblob = nullptr) {
+    return bind_tables<GenericSpace>(p, l, base, gblob);
 }
 
 // ---- ordinal -> plan ---------------------------------------------------------------------------

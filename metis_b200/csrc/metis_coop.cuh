@@ -111,10 +111,11 @@ struct FillState {
 // every subtraction rounded like the reference's) and closes on the first one that does not fit, which is skipped.
 // Only the interval ends fe[] and the residual capacities are written; which stage owns a sub-layer follows from
 // fe[] (CoopEvaluator::vote_coop), so the loop body is a compare and a subtract.
-template <int MAXS, int MAXL>
-MB_HD_NOINLINE FillState seq_forward(const Tables &T, int S, Scratch<MAXS, MAXL> &w) {
+template <int MAXS, int MAXL, class TT>
+MB_HD_NOINLINE FillState seq_forward(const TT &T, int S, Scratch<MAXS, MAXL> &w) {
+    assume_shared_tables(T);
     const int L = T.p.num_layers;
-    const double *dlay = T.dlay;
+    const auto dlay = T.dlay;
     const int N = kH * L;
     const int lim = (N - 1 - kH) > 0 ? (N - 1 - kH) : 0;   // :218
     const int last = S - 1;
@@ -167,10 +168,11 @@ MB_HD_NOINLINE FillState seq_forward(const Tables &T, int S, Scratch<MAXS, MAXL>
 }
 
 // backward pass (:233-249): the last stage takes a contiguous tail [m, N); returns m
-template <int MAXS, int MAXL>
-MB_HD_NOINLINE int seq_backward(const Tables &T, int S, Scratch<MAXS, MAXL> &w, int k) {
+template <int MAXS, int MAXL, class TT>
+MB_HD_NOINLINE int seq_backward(const TT &T, int S, Scratch<MAXS, MAXL> &w, int k) {
+    assume_shared_tables(T);
     const int L = T.p.num_layers;
-    const double *dlay = T.dlay;
+    const auto dlay = T.dlay;
     const int N = kH * L;
     const int last = S - 1;
     double c = w.capa[last];
@@ -216,9 +218,10 @@ MB_HD_NOINLINE int seq_backward(const Tables &T, int S, Scratch<MAXS, MAXL> &w, 
 // empty stages, stages that already hold a leftover).  get_proper_stage: lo = stage of the largest assigned id
 // below j whose stage holds nothing above j, hi = stage of the smallest assigned id above j whose stage holds
 // nothing below j.
-template <int MAXS, int MAXL>
-MB_HD_NOINLINE int seq_skipped(const Tables &T, int S, Scratch<MAXS, MAXL> &w) {
-    const double *dlay = T.dlay;
+template <int MAXS, int MAXL, class TT>
+MB_HD_NOINLINE int seq_skipped(const TT &T, int S, Scratch<MAXS, MAXL> &w) {
+    assume_shared_tables(T);
+    const auto dlay = T.dlay;
     const int last = S - 1;
     int start = 0;                                        // first sub-layer of stage s's forward interval
 #pragma unroll 1
@@ -329,18 +332,18 @@ MB_HD unsigned bucket_of(double u) {
 // Anything else (a bucket holding several entries below t, or a guess above the answer, which monotone rounding
 // rules out) goes to psub_search.  Every branch is uniform: all lanes compute the same values.  Returns i and its
 // entry p = P[i].
-template <class X>
-MB_HD int psub_lookup(const X &x, const double *P, const uint16_t *IX, double scale, int N, int lo, double t, double &p) {
+template <class X, class PT, class IT>
+MB_HD int psub_lookup(const X &x, PT P, IT IX, double scale, int N, int lo, double t, double &p) {
     int i = IX[bucket_of(t * scale)];
     if (i < lo) i = lo;
-    const double *q = P + i;
+    const auto q = P + i;
     const double pm = q[-1], p0 = q[0], p1 = q[1];
     if ((pm < t || i == lo) && p1 >= t) {
         const bool up = !(p0 >= t);
         p = up ? p1 : p0;
         return up ? i + 1 : i;
     }
-    i = psub_search(x, P, N, i, lo, t);
+    i = psub_search(x, tab_generic(P), N, i, lo, t);
     p = P[i];
     return i;
 }
@@ -350,18 +353,19 @@ MB_HD int psub_lookup(const X &x, const double *P, const uint16_t *IX, double sc
 // ---------------------------------------------------------------------------------------------------------
 // ONE = the cluster has a single device type (compile-time: the mixed-type paths are not even instantiated,
 // which halves the code the warps of an SM compete for in the instruction cache)
-template <int MAXS, int MAXL, class X, bool ONE = false>
-struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
-    using Base = PlanEvaluator<MAXS, MAXL, SerialUniform, ONE>;
+template <int MAXS, int MAXL, class X, bool ONE = false, class TT = Tables>
+struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE, TT> {
+    using Base = PlanEvaluator<MAXS, MAXL, SerialUniform, ONE, TT>;
     using Base::T; using Base::w; using Base::pd; using Base::bs_total; using Base::nbad; using Base::aux;
     X x;
     CoopMail &mail;
 
-    MB_HD CoopEvaluator(const Tables &t, Scratch<MAXS, MAXL> &s, CoopMail &mb, const X &lanes)
+    MB_HD CoopEvaluator(const TT &t, Scratch<MAXS, MAXL> &s, CoopMail &mb, const X &lanes)
         : Base(t, s), x(lanes), mail(mb) {}
 
-    // start of every phase: the scratch and the mailbox are the warp's shared memory (X::assume_shared)
-    MB_HD void shared_scratch() const { X::assume_shared(&w); X::assume_shared(&mail); }
+    // start of every phase: the scratch and the mailbox are the warp's shared memory (X::assume_shared), and so is
+    // the descriptor of shared-memory tables (assume_shared_tables)
+    MB_HD void shared_scratch() const { X::assume_shared(&w); X::assume_shared(&mail); assume_shared_tables(T); }
 
     // Start of a plan: groups, rank starts and the first strategy that can be valid (PlanEvaluator::begin,
     // search_space/plan.py:231-249).  The admission pass already dropped plans whose first strategy is invalid.
@@ -486,8 +490,8 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         if (S < 4 || T.p.norm_len < L) { x.note(kPathSeqForward); return false; }   // nothing to overlap: sequential pass
         const int N = kH * L;
         const int lim = (N - 1 - kH) > 0 ? (N - 1 - kH) : 0;  // :218
-        const double *dsub = T.dsub;
-        const double *P = T.psub;
+        const auto dsub = T.dsub;
+        const auto P = T.psub;
         // ---- prediction: uniform walk over the stages ----
         // Stage s starting at a ends at b = min(max(first_ge(P, t) - 1, a), lim), t = perf[s] + P[a]: closed at
         // b < lim exactly when t <= P[lim], and then the next stage starts at i = b + 1 = the first i > a with
@@ -495,7 +499,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         int a = 0, first_open = -1;
         const double scale = T.pidx[0];
         if (scale > 0.0) {                                    // bucket index of psub: a lookup and a check per stage
-            const uint16_t *IX = reinterpret_cast<const uint16_t *>(T.pidx + 1);
+            const auto IX = tab_cast<uint16_t>(T.pidx + 1);
             const double plim = P[lim];
             double pa = P[0];
             int s = 0;
@@ -525,8 +529,8 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
                     const double t = w.perf[s] + P[a];
                     int i0 = a + span - 14;                   // a 32-entry window around the expected end
                     if (i0 < a + 1) i0 = a + 1;
-                    int i = x.first_ge_window(P, N, i0, a + 1, t);
-                    if (i < 0) { x.note(kPathFirstGe); i = x.first_ge(P, N, t); }
+                    int i = x.first_ge_window(tab_generic(P), N, i0, a + 1, t);
+                    if (i < 0) { x.note(kPathFirstGe); i = x.first_ge(tab_generic(P), N, t); }
                     b = i - 1 > a ? i - 1 : a;
                     if (b >= lim) b = lim; else closed = true;
                     span = b - a;
@@ -589,7 +593,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
     MB_HD int fill_coop() {
         shared_scratch();
         const int S = pd.S, last = S - 1;
-        const double *dlay = T.dlay;
+        const auto dlay = T.dlay;
         x.sync();
         const bool fwd = forward_coop();
         x.sync();
@@ -702,7 +706,7 @@ struct CoopEvaluator : PlanEvaluator<MAXS, MAXL, SerialUniform, ONE> {
         const int S = pd.S;
         const int L = T.p.num_layers;
         if (T.p.norm_len < L) return METIS_FATAL_INDEX;       // expand_lc_demand[layer_id] IndexError (:219/:238)
-        const double *lc = T.norm_lc;
+        const auto lc = T.norm_lc;
         const int last = S - 1;
         x.sync();                                            // earlier readers of capa / got are done
         METIS_PAR(x, s, S) { w.capa[s] = w.perf[s]; w.got[s] = 0; }

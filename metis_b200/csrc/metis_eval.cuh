@@ -34,41 +34,96 @@ constexpr int kH = 7;                 // hallucination (model/load_balancer.py:1
 constexpr double kMemCoef = 5.0;      // mem_coef (model/load_balancer.py:31)
 constexpr uint8_t kDropped = 0xFF;    // real layer kept by no stage (quirk Q5)
 
-// Tables as seen by the evaluator (pointers into shared or global memory).
-struct Tables {
+// Where the evaluator reads its tables from, as a type: the address space of the table members of TablesOf.
+// GenericSpace: plain pointers (host build; tables in global memory; the replay kernels).
+struct GenericSpace {
+    template <class V> using ptr = const V *;
+};
+// a typed table pointer reinterpreted as another element type, and as a plain pointer
+template <class U, class V> MB_HD const U *tab_cast(const V *p) { return reinterpret_cast<const U *>(p); }
+template <class V> MB_HD const V *tab_generic(const V *p) { return p; }
+#if defined(__CUDACC__)
+// SharedSpace: the table is in the shared memory of the block, at the 32-bit shared-window address `addr` (the search
+// kernels stage the table blob there, metis_search.cu block_tables).  A read is one LDS with a 32-bit address (base
+// register + immediate), where a generic pointer costs 64-bit address arithmetic and a generic load; the descriptor
+// entry is 4 bytes instead of 8.  Same values, same operations.  The address is complete (it includes the block's
+// window bits), so no read has to rebuild it from the block's shared-memory base.  The loads are PTX: C++ cannot
+// name a shared-memory address as such, and the tables are not written after they are staged.
+__device__ __forceinline__ void lds(uint32_t a, double &v) { asm("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(a)); }
+__device__ __forceinline__ void lds(uint32_t a, int32_t &v) { asm("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a)); }
+__device__ __forceinline__ void lds(uint32_t a, int16_t &v) { asm("ld.shared.s16 %0, [%1];" : "=h"(v) : "r"(a)); }
+__device__ __forceinline__ void lds(uint32_t a, uint16_t &v) { asm("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(a)); }
+__device__ __forceinline__ void lds(uint32_t a, uint8_t &v) {
+    uint32_t r;
+    asm("ld.shared.u8 %0, [%1];" : "=r"(r) : "r"(a));
+    v = (uint8_t)r;
+}
+template <class V>
+struct SmemTab {
+    uint32_t addr;
+    __device__ __forceinline__ V operator[](int i) const {
+        V v;
+        lds(addr + (uint32_t)i * (uint32_t)sizeof(V), v);
+        return v;
+    }
+    template <class I>
+    __device__ __forceinline__ SmemTab operator+(I i) const { return SmemTab{addr + (uint32_t)i * (uint32_t)sizeof(V)}; }
+};
+struct SharedSpace {
+    template <class V> using ptr = SmemTab<V>;
+};
+template <class U, class V> __device__ __forceinline__ SmemTab<U> tab_cast(SmemTab<V> p) { return SmemTab<U>{p.addr}; }
+template <class V> __device__ __forceinline__ const V *tab_generic(SmemTab<V> p) {
+    return static_cast<const V *>(__cvta_shared_to_generic(p.addr));
+}
+#endif
+
+// Tables as seen by the evaluator (in shared or global memory; `Space` above).
+template <class Space>
+struct TablesOf {
+    template <class V> using ptr = typename Space::template ptr<V>;
     MetisProblem p;
-    const int16_t *key_index;
-    const double *lc;          // [num_keys][lpad]
-    const double *mem;         // [num_keys][lpad]
-    const double *exec_full;   // [num_keys]
-    const double *fb_sync;     // [num_keys]
-    const double *norm_lc;     // [norm_len]
-    const double *type_memory, *bw_first, *bw_min;
-    const uint8_t *run_type;   // [ns][num_types]
-    const int32_t *run_end;    // [ns][num_types]  type runs of the true rank -> device map (model/device_group.py:22-32)
-    const int32_t *q10_end;    // [ns][num_types]  type runs of the rank list built with node 0's GPU count (quirk Q10):
+    ptr<int16_t> key_index;
+    ptr<double> lc;            // [num_keys][lpad]
+    ptr<double> mem;           // [num_keys][lpad]
+    ptr<double> exec_full;     // [num_keys]
+    ptr<double> fb_sync;       // [num_keys]
+    ptr<double> norm_lc;       // [norm_len]
+    ptr<double> type_memory, bw_first, bw_min;
+    ptr<uint8_t> run_type;     // [ns][num_types]
+    ptr<int32_t> run_end;      // [ns][num_types]  type runs of the true rank -> device map (model/device_group.py:22-32)
+    ptr<int32_t> q10_end;      // [ns][num_types]  type runs of the rank list built with node 0's GPU count (quirk Q10):
                                //                  load_balancer.py:109-119 (ranks) and cluster_bandwidth.py:158-167 (nodes)
     // derived once per launch (derive_tables): every entry is the result of the same single IEEE
     // operation the reference performs, so looking it up is bit-identical to recomputing it
-    const double *dlay;        // [norm_len] norm_lc[r] / 7              (load_balancer.py:190-193)
-    const double *inv_exec;    // [num_keys] 1. / sum(layer-computes)    (model/device_group.py:80)
-    const double *ratio;       // [num_layers+1] n / num_layers          (cost_estimator.py:146)
-    const double *dpk;         // [kDpk] 2*(dp-1) / (dp * (bw*2^20)), dp = 2^i, uniform bandwidth only (:40-41)
-    const double *pp_hidden;   // [num_bs+1] mbs*seq*hidden / (bw*2^20), uniform bandwidth only (:45-47)
-    const double *pp_vocab;    // [num_bs+1][num_tp] (mbs*seq*vocab / tp) / (bw*2^20)
+    ptr<double> dlay;          // [norm_len] norm_lc[r] / 7              (load_balancer.py:190-193)
+    ptr<double> inv_exec;      // [num_keys] 1. / sum(layer-computes)    (model/device_group.py:80)
+    ptr<double> ratio;         // [num_layers+1] n / num_layers          (cost_estimator.py:146)
+    ptr<double> dpk;           // [kDpk] 2*(dp-1) / (dp * (bw*2^20)), dp = 2^i, uniform bandwidth only (:40-41)
+    ptr<double> pp_hidden;     // [num_bs+1] mbs*seq*hidden / (bw*2^20), uniform bandwidth only (:45-47)
+    ptr<double> pp_vocab;      // [num_bs+1][num_tp] (mbs*seq*vocab / tp) / (bw*2^20)
     // not a reference value: running sum of the sub-layer demands, psub[j] = dlay[0/7] + .. + dlay[(j-1)/7], used only
     // to PREDICT where a stage's forward fill ends (metis_coop.cuh); every prediction is verified exactly
-    const double *psub;        // [7 * num_layers + 1] (empty when norm_len < num_layers)
-    const double *dsub;        // [7 * num_layers] demand of every sub-layer, dsub[j] = dlay[j / 7] (the same bits)
+    ptr<double> psub;          // [7 * num_layers + 1] (empty when norm_len < num_layers)
+    ptr<double> dsub;          // [7 * num_layers] demand of every sub-layer, dsub[j] = dlay[j / 7] (the same bits)
     // bucket index of psub for the prediction (psub_index_entry): pidx[0] = scale (0.0: no index), then the uint16
     // first entries IX[0 .. 7 * num_layers] of the buckets, four per double (empty with psub)
-    const double *pidx;
+    ptr<double> pidx;
     // range sums (fill_range_sums below): rsum[(t * n + b) * n + a] = sum(row_t[a:b]) as CPython adds it up, n =
     // num_layers + 1; rows t: layer_memory of key t, then layer_compute of key t - num_keys, then norm_lc.  Every
     // stage of every candidate needs such a sum (memory demand, execution time, compute left after the vote); the
-    // search kernels look them up, the other kernels (rsum == nullptr) add the slice up.
+    // search kernels look them up, the other kernels (rsum == nullptr) add the slice up.  Always in global memory.
     const double *rsum;
 };
+using Tables = TablesOf<GenericSpace>;
+
+// The descriptor of shared-memory tables is itself in shared memory (one per block, metis_search.cu block_tables).
+// Saying so where an evaluator starts work turns the reads of the descriptor (T.p, the table offsets) into LDS too:
+// the compiler does not infer it through the evaluators' references.  Nothing to say for the other descriptors.
+template <class TT> MB_HD void assume_shared_tables(const TT &) {}
+#if defined(__CUDACC__)
+__device__ __forceinline__ void assume_shared_tables(const TablesOf<SharedSpace> &T) { __builtin_assume(__isShared(&T)); }
+#endif
 
 constexpr int kDpk = 16;
 
@@ -168,7 +223,8 @@ MB_HD double derive_entry(const MetisProblem &p, const DerivedLayout &d, const d
     return ((double)((int64_t)mbs * p.sequence_length * p.vocab_size) / (double)(1 << tpc)) / bw;
 }
 
-MB_HD void bind_derived(Tables &T, const double *base) {
+template <class TT, class B>
+MB_HD void bind_derived(TT &T, B base) {
     const DerivedLayout d = derived_layout(T.p);
     T.dlay = base + d.dlay;
     T.inv_exec = base + d.inv_exec;
@@ -364,9 +420,10 @@ MB_HD const double *range_sum_row(const MetisProblem &p, int t, const double *me
 }
 
 enum RangeTable { kRangeMem = 0, kRangeLc = 1, kRangeNorm = 2 };
-// sum(row[a:b]) of one of the three table families; `row` is the same row in T.mem / T.lc / T.norm_lc
-template <class X>
-MB_HD double range_sum(const Tables &T, int family, int key, const double *row, int a, int b) {
+// sum(row[a:b]) of one of the three table families; `row` is the same row in T.mem / T.lc / T.norm_lc (read through a
+// plain pointer: the search kernels, which stage the tables in shared memory, always find the sum in T.rsum)
+template <class X, class TT, class R>
+MB_HD double range_sum(const TT &T, int family, int key, R row, int a, int b) {
     if (a >= b) return 0.0;
     if (T.rsum && b <= T.p.num_layers) {
         const int n = T.p.num_layers + 1;
@@ -377,7 +434,7 @@ MB_HD double range_sum(const Tables &T, int family, int key, const double *row, 
         return T.rsum[((size_t)t * n + b) * n + a];
 #endif
     }
-    return sum_range<X>(row, a, b);
+    return sum_range<X>(tab_generic(row), a, b);
 }
 
 // Running form of the same sum for values produced on the fly.
@@ -410,10 +467,11 @@ MB_HD double pow2_neg(int k) {
     return d;
 }
 
-MB_HD int type_of_rank(const Tables &T, int ns, int rank) {
+template <class TT>
+MB_HD int type_of_rank(const TT &T, int ns, int rank) {
     const int nt = T.p.num_types;
-    const int32_t *end = T.run_end + ns * nt;
-    const uint8_t *typ = T.run_type + ns * nt;
+    const auto end = T.run_end + ns * nt;
+    const auto typ = T.run_type + ns * nt;
 #pragma unroll 1
     for (int k = 0; k < nt; ++k)
         if (rank < end[k]) return typ[k];
@@ -421,17 +479,19 @@ MB_HD int type_of_rank(const Tables &T, int ns, int rank) {
 }
 
 // device type at position `idx` of the Q10 rank list (callers check idx < T.p.q10_devices)
-MB_HD int type_of_q10(const Tables &T, int ns, int idx) {
+template <class TT>
+MB_HD int type_of_q10(const TT &T, int ns, int idx) {
     const int nt = T.p.num_types;
-    const int32_t *end = T.q10_end + ns * nt;
-    const uint8_t *typ = T.run_type + ns * nt;
+    const auto end = T.q10_end + ns * nt;
+    const auto typ = T.run_type + ns * nt;
 #pragma unroll 1
     for (int k = 0; k < nt; ++k)
         if (idx < end[k]) return typ[k];
     return typ[nt - 1];
 }
 
-MB_HD int key_of(const Tables &T, int type, int tpc, int bs) {
+template <class TT>
+MB_HD int key_of(const TT &T, int type, int tpc, int bs) {
     if (tpc >= T.p.num_tp || bs < 1 || bs > T.p.num_bs) return -1;
     return T.key_index[(type * T.p.num_tp + tpc) * T.p.num_bs + (bs - 1)];
 }
@@ -535,12 +595,13 @@ MB_HD int layer_owner(uint64_t v, bool plurality) {
     return (int)kDropped;
 }
 
-template <int MAXS, int MAXL, class X>
-MB_HD int balance_run(const Tables &T, int S, Scratch<MAXS, MAXL> &w, const X &x) {
+template <int MAXS, int MAXL, class X, class TT>
+MB_HD int balance_run(const TT &T, int S, Scratch<MAXS, MAXL> &w, const X &x) {
+    assume_shared_tables(T);
     const int L = T.p.num_layers;
     if (T.p.norm_len < L) return METIS_FATAL_INDEX;       // expand_lc_demand[layer_id] IndexError (:219/:238)
-    const double *dlay = T.dlay;
-    const double *lc = T.norm_lc;
+    const auto dlay = T.dlay;
+    const auto lc = T.norm_lc;
     const int N = kH * L;
     const int lim = (N - 1 - kH) > 0 ? (N - 1 - kH) : 0;   // :218
     const int last = S - 1;
@@ -838,8 +899,10 @@ struct HSplit {
     int plus[METIS_MAX_TYPES];   // leading replicas of the run that get +1
 };
 
-MB_HD_NOINLINE int partition_data(const Tables &T, int ns, int rank_lo, int count, int dp, int tpc, int bs,
+template <class TT>
+MB_HD_NOINLINE int partition_data(const TT &T, int ns, int rank_lo, int count, int dp, int tpc, int bs,
                                   HSplit &out, uint32_t &aux, bool q10 = false) {
+    assume_shared_tables(T);
     const int gsz = count / dp;
     double perf[METIS_MAX_TYPES];
     PySum total;
@@ -948,9 +1011,10 @@ MB_HD int decode_error(double word, uint32_t &aux) {
     return (int)(code & 0xFF);
 }
 
-template <int MAXS, int MAXL, class X = Serial, bool ONE = false>
+// TT: the tables' type (TablesOf<GenericSpace> or, in the search kernels that stage them, TablesOf<SharedSpace>)
+template <int MAXS, int MAXL, class X = Serial, bool ONE = false, class TT = Tables>
 struct PlanEvaluator {
-    const Tables &T;
+    const TT &T;
     Scratch<MAXS, MAXL> &w;
     X x;
     PlanDesc pd;
@@ -959,7 +1023,7 @@ struct PlanEvaluator {
     uint32_t aux;
     TraceTap *tap;        // verbose transcript only
 
-    MB_HD PlanEvaluator(const Tables &t, Scratch<MAXS, MAXL> &s, const X &lanes = X())
+    MB_HD PlanEvaluator(const TT &t, Scratch<MAXS, MAXL> &s, const X &lanes = X())
         : T(t), w(s), x(lanes), bs_total(0), nbad(0), aux(0), tap(nullptr) {}
 
     MB_HD int group(int s) const { return 1 << w.gcode[s]; }
@@ -980,6 +1044,7 @@ struct PlanEvaluator {
     // If that strategy is invalid it stays invalid for the rest of the chain (mbs and tp only grow).
     // returns 1 ready, 0 plan has no valid strategy, -1 scratch limits exceeded
     MB_HD int begin(const PlanDesc &plan) {
+        assume_shared_tables(T);
         pd = plan;
         if (pd.S > MAXS || T.p.num_layers > MAXL) return -1;
         bs_total = T.p.gbs / pd.batches;
@@ -1036,8 +1101,8 @@ struct PlanEvaluator {
     MB_HD double memory_capacity(int a, int b) const {
         const int nt = T.p.num_types;
         if (ONE || nt == 1) return T.type_memory[0] * (double)(b - a);
-        const int32_t *end = T.run_end + pd.ns * nt;
-        const uint8_t *typ = T.run_type + pd.ns * nt;
+        const auto end = T.run_end + pd.ns * nt;
+        const auto typ = T.run_type + pd.ns * nt;
         PySum acc;
         int lo = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -1067,6 +1132,7 @@ struct PlanEvaluator {
 
     // mixed-type stage of get_intra_stage_compute_performance (model/device_group.py:68-76)
     MB_HD_NOINLINE int hetero_performance(int a, int b, int dp, int tpc, double &p) {
+        assume_shared_tables(T);
         HSplit hs;
         int rc = partition_data(T, pd.ns, a, b - a, dp, tpc, bs_total, hs, aux);
         if (rc) return rc;
@@ -1224,6 +1290,7 @@ struct PlanEvaluator {
 
     // StagePerformance.get_intra_stage_compute_performance (model/device_group.py:54-85) -> w.perf
     MB_HD int compute_performance() {
+        assume_shared_tables(T);
         PySum total;
         int rc = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -1245,6 +1312,7 @@ struct PlanEvaluator {
 
     // mixed-type stage of _get_stage_memory_demand (model/load_balancer.py:45-52, quirk Q6)
     MB_HD_NOINLINE int hetero_memory_demand(int s, int type0, double &demand) {
+        assume_shared_tables(T);
         const int la = w.part[s], lb = w.part[s + 1], tpc = w.tpc[s];
         HSplit hs;                                           // whole-cluster device list (quirk Q6)
         const int rc = partition_data(T, pd.ns, 0, T.p.q10_devices, dp_of(s), tpc, bs_total, hs, aux, true);
@@ -1269,6 +1337,7 @@ struct PlanEvaluator {
     // Opt-in METIS_FIX_Q6 (NOT the reference; mirrored by oracle.stage_memory_demand_own_type): the stage's own
     // devices decide the memory profile; a mixed-type stage needs the memory of its largest replica.
     MB_HD_NOINLINE int memory_demand_own_type(int s, double &demand) {
+        assume_shared_tables(T);
         const int la = w.part[s], lb = w.part[s + 1], tpc = w.tpc[s], g = w.gcode[s];
         const int a = rank_start(s), b = a + (1 << g);
         const int ta = type_of_rank(T, pd.ns, a), tb = type_of_rank(T, pd.ns, b - 1);
@@ -1309,6 +1378,7 @@ struct PlanEvaluator {
     // in: w.perf (c_capa), w.extra (m_demand); out: w.perf; returns 1 = None, 0 ok, <0 fatal (negated code)
     // w.extra is overwritten on both returns (additional_alloc_sc_capa; zero when the result is None)
     MB_HD_NOINLINE int adjust_performance() {
+        assume_shared_tables(T);
         const int S = pd.S;
         double need = 0.;
         PySum avail_sum;
@@ -1362,6 +1432,7 @@ struct PlanEvaluator {
     }
     template <class Sink>
     MB_HD int memory_phase(int attempt, Sink &sink) {
+        assume_shared_tables(T);
         const int S = pd.S;
         bool oom = false;
         int rc = 0;
@@ -1399,6 +1470,7 @@ struct PlanEvaluator {
     // returns attempt number 1..3, 0 = (None, -1, None), <0 = fatal (negated code)
     template <class Sink>
     MB_HD_NOINLINE int partition_layer(Sink &sink) {
+        assume_shared_tables(T);
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int attempt = 1; attempt <= 3; ++attempt) {
             sink.balancer_run();
@@ -1417,8 +1489,8 @@ struct PlanEvaluator {
         if (n0 == n1) return T.bw_first[type_of_q10(T, pd.ns, n0 * per)];
         double slow = INFINITY;
         const int nt = T.p.num_types;
-        const int32_t *end = T.q10_end + pd.ns * nt;
-        const uint8_t *typ = T.run_type + pd.ns * nt;
+        const auto end = T.q10_end + pd.ns * nt;
+        const auto typ = T.run_type + pd.ns * nt;
         int lo = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
         for (int k = 0; k < nt; ++k) {                       // types whose node run intersects [n0, n1]
@@ -1457,6 +1529,7 @@ struct PlanEvaluator {
 
     // mixed-type stage of _get_execution_cost (model/cost_estimator.py:189-197 with :152-173)
     MB_HD_NOINLINE int hetero_exec_cost(int a, int b, int dp, int tpc, int la, int lb, double &len) {
+        assume_shared_tables(T);
         HSplit hs;
         uint32_t dummy;
         if (partition_data(T, pd.ns, a, b - a, dp, tpc, bs_total, hs, dummy)) return 1;
@@ -1486,8 +1559,8 @@ struct PlanEvaluator {
     // _get_fb_sync_cost over the device types of ranks [a, b) (model/cost_estimator.py:57-72, quirk Q9)
     MB_HD int fb_sync_cost(int a, int b, int tpc, int mbs, double &out) const {
         const int nt = T.p.num_types;
-        const int32_t *end = T.run_end + pd.ns * nt;
-        const uint8_t *typ = T.run_type + pd.ns * nt;
+        const auto end = T.run_end + pd.ns * nt;
+        const auto typ = T.run_type + pd.ns * nt;
         double mx = -INFINITY;
         int lo = 0;
 #pragma unroll (X::kUniform ? 1 : 0)
@@ -1508,6 +1581,7 @@ struct PlanEvaluator {
 
     // HeteroCostEstimator.get_cost (model/cost_estimator.py:199-244); returns 0 ok, 1 KeyError.
     MB_HD int get_cost(double &cost_out) {
+        assume_shared_tables(T);
         const bool one_type = ONE || T.p.num_types == 1;
         const int nstage = pd.label < pd.S ? pd.label : pd.S;  // zip(range(plan.num_stage), strategies)
         // rank_node_map holds num_nodes * devices(node 0) ranks (cluster_bandwidth.py:34-47, Q10): a costed stage
@@ -1602,12 +1676,13 @@ struct PlanEvaluator {
 // returns true when the plan continues in the chain kernel; `chain_hint` then estimates how long its chain is
 // (PlanEvaluator::halvings; used only to start long chains first).
 // ---------------------------------------------------------------------------
-template <int MAXS, int MAXL, bool ONE, class X = Serial, class Sink>
-MB_HD bool first_task(const Tables &T, Scratch<MAXS, MAXL> &w, Sink &sink, bool has, const PlanDesc &plan, int &chain_hint,
+template <int MAXS, int MAXL, bool ONE, class X = Serial, class Sink, class TT>
+MB_HD bool first_task(const TT &T, Scratch<MAXS, MAXL> &w, Sink &sink, bool has, const PlanDesc &plan, int &chain_hint,
                       int &resume) {
+    assume_shared_tables(T);
     // X = Lockstep (device, called by all 32 lanes of a warp, with or without a plan): the lanes are re-joined
     // between the phases and inside the balancer.  X = Serial: one thread on its own.
-    PlanEvaluator<MAXS, MAXL, X, ONE> ev(T, w);
+    PlanEvaluator<MAXS, MAXL, X, ONE, TT> ev(T, w);
     bool cont = false;
     sink.phase(1);
     if (has) {                                               // ---- P ----

@@ -160,12 +160,24 @@ __device__ __forceinline__ void stage_blob_tma(uint8_t *smem, const uint8_t *blo
     }
 }
 
-// Tables of a search kernel: one descriptor per block, in shared memory, written by thread 0 while the tables are
-// staged.  A copy per thread (the whole MetisProblem and the table pointers, ~430 B) would live in local memory,
-// and every read of a launch constant (T.p.num_layers, T.rsum, ...) would be a local load.  Called by all threads.
-__device__ __forceinline__ const Tables &block_tables(Tables &s_tables, const MetisProblem &p, const BlobLayout &lay,
-                                                      const uint8_t *blob, uint8_t *smem, int use_smem, uint64_t *mbar) {
-    if (threadIdx.x == 0) s_tables = make_tables(p, lay, use_smem ? smem : blob, blob);
+// Tables of a search kernel: staged into the kernel's dynamic shared memory `smem` when `use_smem` is set, else read
+// from the blob in global memory.  Template flag SMEM (only with use_smem): the reads are shared loads with 32-bit
+// addresses (SharedSpace, metis_eval.cuh), else plain pointers (GenericSpace).  One descriptor per block, in shared
+// memory, written by thread 0 while the tables are staged.
+// A copy per thread (the whole MetisProblem and the table addresses, ~350 B) would live in local memory, and every
+// read of a launch constant (T.p.num_layers, T.rsum, ...) would be a local load.  Called by all threads.
+template <bool SMEM>
+using SearchTables = TablesOf<typename std::conditional<SMEM, SharedSpace, GenericSpace>::type>;
+
+template <bool SMEM>
+__device__ __forceinline__ const SearchTables<SMEM> &block_tables(SearchTables<SMEM> &s_tables, const MetisProblem &p,
+                                                                  const BlobLayout &lay, const uint8_t *blob,
+                                                                  uint8_t *smem, int use_smem, uint64_t *mbar) {
+    if constexpr (SMEM) {
+        if (threadIdx.x == 0) s_tables = bind_tables<SharedSpace>(p, lay, SmemTab<uint8_t>{smem_u32(smem)}, blob);
+    } else {
+        if (threadIdx.x == 0) s_tables = make_tables(p, lay, use_smem ? smem : blob, blob);
+    }
     if (use_smem) stage_blob_tma(smem, blob, lay.total, mbar);     // its __syncthreads publishes s_tables
     else __syncthreads();
     return s_tables;
@@ -467,7 +479,7 @@ het_scatter_kernel(const SearchLists ls) {
     }
 }
 
-template <int MAXS, int MAXL, bool ONE, int OUT>
+template <int MAXS, int MAXL, bool ONE, int OUT, bool SMEM>
 __global__ void __launch_bounds__(kThreads, (MAXS <= 64 ? METIS_MIN_BLOCKS : ONE ? METIS_MIN_BLOCKS_BIG_ONE : METIS_MIN_BLOCKS_BIG))
 het_first_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ MetisPlanSpace sp,
                  const __grid_constant__ BlobLayout lay, const uint8_t *__restrict__ blob, const int use_smem,
@@ -475,11 +487,11 @@ het_first_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
                  const MissOut misses) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
-    __shared__ Tables s_tables;
+    __shared__ SearchTables<SMEM> s_tables;
     auto sink = make_sink<OUT>(out, headroom, misses);
     const unsigned int n = ls.ctl[0];
     if ((long long)n >= ls.bulk_min) {
-        const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
+        const auto &T = block_tables<SMEM>(s_tables, p, lay, blob, smem, use_smem, &mbar);
         Scratch<MAXS, MAXL> w;
         if constexpr ((OUT & kOutHeadroom) != 0) sink.state = w.mstate;
         const int lane = threadIdx.x & 31;
@@ -549,7 +561,7 @@ struct alignas(16) ChainScratch {
 
 
 // 64 registers per thread: 32 resident warps per SM in blocks of 16 warps (tables staged once per block)
-template <int MAXS, int MAXL, bool ONE, int OUT>
+template <int MAXS, int MAXL, bool ONE, int OUT, bool SMEM>
 __global__ void __launch_bounds__(512, 2)
 het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__ MetisPlanSpace sp,
                  const __grid_constant__ BlobLayout lay, const uint8_t *__restrict__ blob, const int use_smem,
@@ -557,9 +569,9 @@ het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
                  const int best_slot, double *headroom, const MissOut misses) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t mbar;
-    __shared__ Tables s_tables;
+    __shared__ SearchTables<SMEM> s_tables;
     WarpCoop::prof_init();                                   // (phase clock build only; published by block_tables)
-    const Tables &T = block_tables(s_tables, p, lay, blob, smem, use_smem, &mbar);
+    const auto &T = block_tables<SMEM>(s_tables, p, lay, blob, smem, use_smem, &mbar);
     auto sink = make_sink<OUT>(out, headroom, misses);
     const int lane = threadIdx.x & 31;
     sink.leader = lane == 0;
@@ -570,7 +582,7 @@ het_chain_kernel(const __grid_constant__ MetisProblem p, const __grid_constant__
     const uint4 *list = ls.b;                                // sorted: by chain hint after a bulk round, else by stage count
     const unsigned int n = bulk ? ls.ctl[2] : n_adm;
     ChainCoop lanes;
-    CoopEvaluator<MAXS, MAXL, ChainCoop, ONE> ev(T, cs->w, cs->mail, lanes);
+    CoopEvaluator<MAXS, MAXL, ChainCoop, ONE, SearchTables<SMEM>> ev(T, cs->w, cs->mail, lanes);
     for (;;) {
         unsigned int i = 0;
         if (lane == 0) i = atomicAdd(&ls.ctl[3], 1u);
@@ -918,6 +930,10 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     if (sms < 1 || smem_optin < 48 * 1024) return cuda_fail(cudaErrorInvalidDevice, "device attributes");
     const int blob_max = env_int("METIS_SMEM_BLOB_MAX", 0, kSmemBlobMax, kSmemBlobMax);   // larger tables stay in global memory
+    // Staged tables read with shared loads (SharedSpace) only on single-type clusters: C3-mpl6 (one type) measured 3 %
+    // faster with them, c4_het128_mpl6 (two types) 3 % slower, so mixed-type clusters keep plain pointers to the staged
+    // tables, and the search kernels exist in that form only once (DESIGN.md section 5).
+    constexpr bool SHARED = ONE;
     const unsigned int blob_pad = (lay.total + 127u) & ~127u;
 
     SearchLists ls;
@@ -930,7 +946,10 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     ls.save_cap = (unsigned int)save_slots(cap);
 
     // ---- chain kernel: warps per block chosen so that tables + per-warp scratch fill the SM with warps ----
-    auto chain = het_chain_kernel<MAXS, MAXL, ONE, OUT>;
+    // (staged tables are read with shared loads on single-type clusters, SHARED below, else through plain pointers)
+    auto chain_kernel = [](int smem_tables) {
+        return smem_tables ? het_chain_kernel<MAXS, MAXL, ONE, OUT, SHARED> : het_chain_kernel<MAXS, MAXL, ONE, OUT, false>;
+    };
     const size_t per_warp = sizeof(ChainScratch<MAXS, MAXL>);
     int chain_smem_tables = (int)lay.total <= blob_max;
     int chain_threads = 0, chain_per_sm = 0;
@@ -938,6 +957,7 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
     unsigned int chain_off = 0;
     const int forced = env_int("METIS_CHAIN_THREADS", 32, 512, 0);
     for (int pass = 0; pass < 2 && chain_threads == 0; ++pass) {       // second pass: tables in global memory
+        const auto chain = chain_kernel(chain_smem_tables);
         int best_warps = 0;
         for (int threads = 64; threads <= 512; threads *= 2) {
             if (forced && threads != ((forced + 31) & ~31)) continue;
@@ -956,16 +976,25 @@ static int launch_search(const MetisProblem &p_arg, const MetisPlanSpace &s_arg,
         if (chain_threads == 0) chain_smem_tables = 0;
     }
     if (chain_threads == 0) return arg_fail("chain kernel does not fit this device (shared memory)");
+    const auto chain = chain_kernel(chain_smem_tables);
     e = cudaFuncSetAttribute(chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chain_dyn);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(chain)");
     int64_t chain_grid = (int64_t)sms * chain_per_sm;
 
     // ---- bulk round ----
-    auto first = het_first_kernel<MAXS, MAXL, ONE, OUT>;
+    auto first = het_first_kernel<MAXS, MAXL, ONE, OUT, SHARED>;
     int first_smem_tables = (int)lay.total <= blob_max && blob_pad <= (unsigned int)smem_optin;
-    size_t first_dyn = first_smem_tables ? blob_pad : 0;
-    e = cudaFuncSetAttribute(first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_dyn);
-    if (e != cudaSuccess) { cudaGetLastError(); first_smem_tables = 0; first_dyn = 0; }   // static + blob too large
+    size_t first_dyn = blob_pad;
+    if (first_smem_tables) {
+        e = cudaFuncSetAttribute(first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)first_dyn);
+        if (e != cudaSuccess) { cudaGetLastError(); first_smem_tables = 0; }   // static + blob too large
+    }
+    if (!first_smem_tables) {                                // tables in global memory
+        first = het_first_kernel<MAXS, MAXL, ONE, OUT, false>;
+        first_dyn = 0;
+        e = cudaFuncSetAttribute(first, cudaFuncAttributeMaxDynamicSharedMemorySize, 0);
+        if (e != cudaSuccess) cudaGetLastError();
+    }
     int first_per_sm = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&first_per_sm, first, kThreads, first_dyn);
     if (e != cudaSuccess || first_per_sm < 1) return cuda_fail(e, "occupancy query (bulk round)");

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Developer tool: static count of the local-memory instructions (LDL / STL) of a search kernel, by phase of the
-bulk round.
+"""Developer tool: static count of the local-memory instructions (LDL / STL) and generic loads (LD) of a search
+kernel, by phase of the bulk round.
 
   python tools/sass_phases.py [kernel-substring] [--lib PATH | --cubin PATH]
 
@@ -8,8 +8,10 @@ The library is built with -lineinfo, so `nvdisasm -gi` gives every SASS instruct
 inlined calls that led there.  An instruction belongs to the innermost frame that lies in one of the evaluator's
 drivers in metis_eval.cuh (PlanEvaluator::begin / compute_performance / memory_phase / adjust_performance / get_cost,
 balance_run cut at its x.mark() hooks); the out-of-line helpers count for the phase that calls them.  Printed per
-phase: instructions, LDL and STL.  Together with the phase clock (tools/phase_profile.py --bulk) this says which
-phase's scratch traffic is worth cutting; it counts code, not executions.
+phase: instructions, LDL, STL and LD.  Together with the phase clock (tools/phase_profile.py --bulk) this says which
+phase's scratch traffic is worth cutting; it counts code, not executions.  In the instantiations that read the tables
+from shared memory (template flag SMEM) a generic LD is never a table read on a common path: a table or descriptor
+read that shows up here lost its shared-memory hint (metis_eval.cuh, assume_shared_tables).
 """
 import argparse
 import collections
@@ -96,7 +98,7 @@ def main():
             name = ln.split('.text.', 1)[1].split()[0]
             name = name if ns.kernel in name else None
             if name:
-                per[name] = collections.defaultdict(lambda: [0, 0, 0])
+                per[name] = collections.defaultdict(lambda: [0, 0, 0, 0])
             continue
         if name is None:
             continue
@@ -114,16 +116,17 @@ def main():
             row[0] += 1
             row[1] += op == 'LDL'
             row[2] += op == 'STL'
+            row[3] += op == 'LD'
     if not per:
         raise SystemExit(f'no kernel matches {ns.kernel!r}')
     for name, rows in per.items():
-        tot = [sum(r[k] for r in rows.values()) for k in range(3)]
-        print(f'{name}: {tot[0]} instructions, {tot[1]} LDL, {tot[2]} STL')
-        print(f'  {"phase":<14s} {"instr":>6s} {"LDL":>5s} {"STL":>5s}')
+        tot = [sum(r[k] for r in rows.values()) for k in range(4)]
+        print(f'{name}: {tot[0]} instructions, {tot[1]} LDL, {tot[2]} STL, {tot[3]} LD')
+        print(f'  {"phase":<14s} {"instr":>6s} {"LDL":>5s} {"STL":>5s} {"LD":>5s}')
         for ph in ORDER:
             if ph in rows:
                 r = rows[ph]
-                print(f'  {ph:<14s} {r[0]:6d} {r[1]:5d} {r[2]:5d}')
+                print(f'  {ph:<14s} {r[0]:6d} {r[1]:5d} {r[2]:5d} {r[3]:5d}')
 
 
 if __name__ == '__main__':
