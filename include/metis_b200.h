@@ -334,6 +334,37 @@ int metis_recost_regret(const double *costs, int32_t num_scenarios, int64_t n, d
                         void *workspace, int64_t workspace_bytes, void *stream);
 
 /*
+ * Profile what-if: costed candidates of one search under other profiles, with their device groups, strategies and
+ * layer partition held fixed (no strategy chain, no balancer run: not what a search under the scenario returns).
+ * For scenario j, record i:
+ *   costs[j * n + i]    HeteroCostEstimator.get_cost (model/cost_estimator.py:199-244) under scenario j's tables;
+ *                       NaN when it raises
+ *   headroom[j * n + i] min over all S stages of memory capacity - LayerLoadBalancer._get_stage_memory_demand
+ *                       (model/load_balancer.py:29-55, quirks Q6 and Q10) under scenario j; NaN when the demand raises
+ *   status[j * n + i]   cost_code | memory_code << 4, each METIS_FATAL_NONE or a METIS_FATAL_* code: cost_code is
+ *                       METIS_FATAL_KEY_EXEC whenever get_cost raises; memory_code is the first failing stage's
+ *                       METIS_FATAL_KEY_MEMORY / KEY_EXEC (a missing key), METIS_FATAL_INDEX (Q10) or
+ *                       METIS_FATAL_ZERODIV (the data split of a mixed-type stage)
+ *   A candidate is usable under scenario j when status == 0 and headroom >= 0.
+ * Each scenario is a MetisProblem flattened from a profile under the searched cluster, model flags and corrections:
+ * its profile tables (keys, num_bs, lpad, ...) may differ, its scalar fields outside the profile must equal
+ * scenarios[0]'s (num_types, num_layers, gbs, num_nodes, devices_per_node, total_devices, num_node_sequences,
+ * q10_devices, uniform_bw, corrected; otherwise METIS_E_ARG).  Its cluster tables (memory, bandwidth, node sequence
+ * runs) are not compared: the caller builds every scenario from the searched cluster.  Under the searched profile,
+ * costs and headroom equal the search's, bit for bit.
+ *   space      the searched plan space;  records [device] n MetisRecord of it (any order), only ordinal is read
+ *   detail     [device] n rows of detail_stride bytes, as for metis_het_recost; detail_stride >= 3 * max_stage + 1
+ *   costs, headroom [device] num_scenarios x n doubles;  status [device] num_scenarios x n bytes
+ *   1 <= num_scenarios <= 65535;  workspace [device] metis_het_profile_recost_workspace_bytes(scenarios, num_scenarios)
+ *   bytes (METIS_E_CAPACITY when smaller), laid out as the scenarios' descriptors, then each one's packed tables
+ */
+int64_t metis_het_profile_recost_workspace_bytes(const MetisProblem *scenarios, int32_t num_scenarios);
+int metis_het_profile_recost(const MetisPlanSpace *space, const MetisProblem *scenarios, int32_t num_scenarios,
+                             const MetisRecord *records, int64_t n, const uint8_t *detail, int32_t detail_stride,
+                             double *costs, double *headroom, uint8_t *status,
+                             void *workspace, int64_t workspace_bytes, void *stream);
+
+/*
  * metis_homo_cost with the cost terms and the per-stage memory sums (HomoCostEstimator.get_cost returns them as
  * stage_memory, model/cost_estimator.py:121-138).
  *   terms        [device] n x 6 doubles: execution, fb_sync, parameter update, dp, pp, batch generate

@@ -186,6 +186,9 @@ class HetSearchResult(Sequence):
         self._ranker = ranker                 # () -> uint32 permutation, the stable device sort by cost
         self._best_key = best_key             # (ordinal, step) of the argmin found by the search kernels
         self._searched = None                 # cluster_signature of the cluster searched (cost_het_cluster sets it)
+        # (cluster, model_config, gbs, max_tp, max_bs, node_sequences, corrected) the search flattened its profile
+        # under (cost_het_cluster sets it): a profile what-if flattens its scenarios the same way
+        self._flat_inputs = None
 
     def __len__(self) -> int:
         return len(self.candidates)
@@ -435,6 +438,36 @@ class HetSearchResult(Sequence):
             bw[j, 0], bw[j, 1] = flatten.cluster_bandwidths(cluster, type_names, corrected)
         return self.candidates.recost(bw)
 
+    def recost_profiles(self, profiles: Sequence[Dict]) -> 'search.Recost':
+        """Profile what-if: every candidate, with its device groups, strategies and layer partition held fixed, under
+        each profile of ``profiles`` (dicts shaped like ProfileDataLoader.load_profile_data_all()[0]) on the GPU
+        (metis_het_profile_recost).  For scenario j: ``costs[j]`` is HeteroCostEstimator.get_cost
+        (model/cost_estimator.py:199-244) under profile j, ``headroom[j]`` the smallest memory capacity -
+        LayerLoadBalancer._get_stage_memory_demand (model/load_balancer.py:29-55) over all stages under profile j, and
+        ``status[j]`` cost code | memory code << 4 (METIS_FATAL_*; a raising get_cost is METIS_FATAL_KEY_EXEC); a
+        candidate is ``usable`` under j when status == 0 and headroom >= 0.  This is not what a search under profile j
+        returns: a search would re-run the strategy chain and the balancer and pick other partitions.  Under the
+        searched profile, costs and headroom equal the search's bit for bit.  The corrections of the search apply to
+        every scenario.  A profile without a 'model' section holding parameters, optimizer_time and batch_generator,
+        or without an entry for a device type of the cluster, is refused with a ValueError; wrong values are not:
+        they become statuses, as they would be errors in the reference.  Returns a search.Recost whose ``ranked(j, k)``
+        and ``best(j)`` list the candidates usable under j by scenario cost, and whose ``regret`` and ``robust(k)``
+        take unusable entries as +inf.  With torch.distributed every rank holds all candidates: no collective is
+        issued."""
+        if self._flat_inputs is None:
+            raise ValueError('this result does not know the inputs it was searched on: no recost_profiles')
+        profiles = list(profiles)
+        if not profiles:
+            raise ValueError('recost_profiles needs at least one profile')
+        cluster, model_config, gbs, max_tp, max_bs, seqs, corrected = self._flat_inputs
+        problem = self.candidates.problem
+        for j, prof in enumerate(profiles):
+            check_profile(prof, problem.type_names, j)
+        norm = problem.arrays['norm_lc']                      # read by the balancer only, which does not run here
+        scen = [flatten.build_problem(prof, cluster, model_config, gbs, max_tp, max_bs, seqs, norm, corrected=corrected)
+                for prof in profiles]
+        return self.candidates.recost_profiles(scen)
+
     def best(self) -> Optional[Tuple]:
         """argmin (cost, position): the first entry of the ranked list.  The search kernels reduce it on the device
         (het_finalize_kernel: lowest cost, then lowest ordinal, then lowest step), so no sort is needed for it."""
@@ -458,6 +491,24 @@ def cluster_signature(gpu_cluster, type_names: Sequence[str]) -> Tuple[list, lis
 
 
 _NODE_FIELDS = ('ip', 'GPU count', 'instance_type', 'memory')
+_MODEL_FIELDS = ('parameters', 'optimizer_time', 'batch_generator')
+
+
+def check_profile(profile, type_names: Sequence[str], j: int) -> None:
+    """ValueError, naming scenario j and the missing item, unless ``profile`` has a 'model' section with parameters,
+    optimizer_time and batch_generator and an entry for every device type of ``type_names``."""
+    if not isinstance(profile, dict):
+        raise ValueError(f'profile {j}: a dict like ProfileDataLoader.load_profile_data_all()[0], not '
+                         f'{type(profile).__name__}')
+    model = profile.get('model')
+    if not isinstance(model, dict):
+        raise ValueError(f"profile {j}: no 'model' section")
+    for field in _MODEL_FIELDS:
+        if field not in model:
+            raise ValueError(f"profile {j}: the 'model' section has no {field!r}")
+    for name in type_names:
+        if not isinstance(profile.get(f'DeviceType.{name}'), dict):
+            raise ValueError(f'profile {j}: no DeviceType.{name} entry for device type {name} of the cluster')
 
 
 def check_scenario(searched: Tuple[list, list], cluster, type_names: Sequence[str], corrected: Sequence[str],
@@ -640,6 +691,8 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     if misses:
         result.timings['misses_s'] = out.misses_s
     result._searched = cluster_signature(gpu_cluster, problem.type_names)
+    result._flat_inputs = (gpu_cluster, model_config, args.gbs, args.max_profiled_tp_degree,
+                           args.max_profiled_batch_size, [tuple(s) for s in node_sequences], tuple(corrected))
     return result
 
 

@@ -116,4 +116,7 @@ __device__ __forceinline__ bool decode_plan(const MetisPlanSpace &sp, int64_t or
 int stage_replay_tables(const MetisProblem *problem, void *workspace, int64_t workspace_bytes, cudaStream_t stream,
                         BlobLayout &lay, const uint8_t *&blob);
 
+// The workspace bytes stage_replay_tables needs for `problem`, or METIS_E_ARG.  Defined in metis_search.cu.
+int64_t replay_tables_bytes(const MetisProblem *problem);
+
 }  // namespace metis

@@ -19,8 +19,9 @@ struct RecostEvaluator : PlanEvaluator<MAXS, MAXL> {
     int nstage;
     double exec, fb_sync, max_upd, bg;
 
-    // `t` must read its bandwidths through the general path (t.p.uniform_bw == 0): its bw_first / bw_min hold the
-    // scenario when scenario_cost is called
+    // For the bandwidth what-if (metis_het_recost), `t` must read its bandwidths through the general path
+    // (t.p.uniform_bw == 0): its bw_first / bw_min hold the scenario when scenario_cost is called.  The profile what-if
+    // (metis_profile.cu) binds `t` to a whole scenario's tables, derived bandwidth tables included.
     MB_HD RecostEvaluator(const Tables &t, Scratch<MAXS, MAXL> &s) : Base(t, s), nstage(0), exec(0), fb_sync(0), max_upd(0), bg(0) {}
 
     // The candidate: plan `plan` with the strategies and partition of its detail row (dp codes[S], tp codes[S],

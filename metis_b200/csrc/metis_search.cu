@@ -1150,13 +1150,18 @@ int metis_het_detail(const MetisProblem *problem, const MetisPlanSpace *space, c
 
 }  // extern "C"
 
+int64_t metis::replay_tables_bytes(const MetisProblem *problem) {
+    if (check_problem(problem)) return METIS_E_ARG;
+    return 256 + kFixedWs + (int64_t)align16(make_layout(*problem).total);
+}
+
 int metis::stage_replay_tables(const MetisProblem *problem, void *workspace, int64_t workspace_bytes, cudaStream_t stream,
                                BlobLayout &lay, const uint8_t *&blob) {
-    int rc = check_problem(problem);
-    if (rc) return rc;
+    const int64_t need = replay_tables_bytes(problem);
+    if (need < 0) return (int)need;
     if (!workspace) return arg_fail("NULL argument");
     lay = make_layout(*problem);
-    if (workspace_bytes < 256 + kFixedWs + (int64_t)align16(lay.total)) return METIS_E_CAPACITY;
+    if (workspace_bytes < need) return METIS_E_CAPACITY;
     const Workspace ws = carve(workspace, lay);
     pack_tables_kernel<<<8, 256, 0, stream>>>(*problem, lay, ws.blob);
     blob = ws.blob;

@@ -107,7 +107,8 @@ SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 
            'metis_enum_compositions', 'metis_generate_rows', 'metis_list_workspace_bytes', 'metis_list_stages',
            'metis_list_window', 'metis_het_search_headroom', 'metis_headroom_workspace_bytes', 'metis_headroom_select',
            'metis_headroom_front', 'metis_het_search_outputs', 'metis_het_recost', 'metis_recost_regret_workspace_bytes',
-           'metis_recost_regret', 'metis_query_mark', 'metis_query_groups', 'metis_mask_select']
+           'metis_recost_regret', 'metis_query_mark', 'metis_query_groups', 'metis_mask_select',
+           'metis_het_profile_recost_workspace_bytes', 'metis_het_profile_recost']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -171,6 +172,12 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_recost_regret.restype = C.c_int
     lib.metis_recost_regret.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_void_p]
+    lib.metis_het_profile_recost_workspace_bytes.restype = C.c_int64
+    lib.metis_het_profile_recost_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
+    lib.metis_het_profile_recost.restype = C.c_int
+    lib.metis_het_profile_recost.argtypes = [C.POINTER(MetisPlanSpace), C.c_void_p, C.c_int32, C.c_void_p, C.c_int64,
+                                             C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_int64, C.c_void_p]
     lib.metis_query_mark.restype = C.c_int
     lib.metis_query_mark.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisPlanFilter),
                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_void_p,

@@ -36,10 +36,10 @@ def upload(a: np.ndarray, device) -> torch.Tensor:
 
 
 def bind_problem(problem: flatten.FlatProblem, device, space: Optional[flatten.FlatPlanSpace] = None,
-                 rows: Optional[torch.Tensor] = None):
+                 rows: Optional[torch.Tensor] = None, workspace: bool = True):
     """``problem``'s tables (and ``space``'s blocks and batches, with ``rows``, its device-group rows on ``device``)
-    uploaded to ``device``: (lib, problem struct, space struct or None, a workspace for the replay kernels, the tensors
-    the structs point into)."""
+    uploaded to ``device``: (lib, problem struct, space struct or None, a workspace for the replay kernels (None
+    without ``workspace``), the tensors the structs point into)."""
     lib = native.load_library()
     with torch.cuda.device(device):
         tens = {k: upload(v, device) for k, v in problem.arrays.items()}
@@ -47,7 +47,8 @@ def bind_problem(problem: flatten.FlatProblem, device, space: Optional[flatten.F
             tens.update(blocks=upload(space.blocks, device), batches=upload(space.batches, device), rows=rows)
         p = problem.as_struct(lambda n: tens[n].data_ptr())
         sp = space.as_struct(lambda n: tens[n].data_ptr()) if space is not None else None
-        ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=device)
+        ws = torch.empty(int(lib.metis_het_workspace_bytes(C.byref(p), 0, 1)), dtype=torch.uint8, device=device) \
+            if workspace else None
     return lib, p, sp, ws, tens
 
 
@@ -665,6 +666,45 @@ class Candidates:
         t2 = time.perf_counter()
         return Recost(self, costs, best, regret, dev, {'recost_s': t1 - t0, 'regret_s': t2 - t1})
 
+    def recost_profiles(self, problems: Sequence[flatten.FlatProblem]) -> 'Recost':
+        """Every candidate under the scenario profiles ``problems`` (each flattened under the searched cluster, model
+        flags and corrections), with its device groups, strategies and partition held fixed: cost, headroom and status
+        per scenario (metis_het_profile_recost), segment by segment, _RECOST_CHUNK records per launch.  The scenarios'
+        tables are uploaded once.  timings: ``recost_s`` up to the arrays on the host, ``regret_s`` the regret kernels
+        and their copy."""
+        t0 = time.perf_counter()
+        dev = _require_cuda(self.device)
+        K, n = len(problems), len(self.records)
+        with torch.cuda.device(dev):
+            bound = [bind_problem(pr, dev, workspace=False) for pr in problems]
+            lib = bound[0][0]
+            scen = (native.MetisProblem * K)(*[b[1] for b in bound])
+            need = int(lib.metis_het_profile_recost_workspace_bytes(C.c_void_p(C.addressof(scen)), C.c_int32(K)))
+            native.check(min(need, 0), 'metis_het_profile_recost_workspace_bytes')
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            costs_dev = torch.empty((K, n), dtype=torch.float64, device=dev)
+            head_dev = torch.empty((K, n), dtype=torch.float64, device=dev)
+            status_dev = torch.empty((K, n), dtype=torch.uint8, device=dev)
+            for seg in self.segments:
+                if seg.first == seg.end:                      # nothing to replay: a window is not reloaded for it
+                    continue
+                _lib, _p, sp, _ws, _dev, _keep = seg.bind()
+                for lo in range(seg.first, seg.end, _RECOST_CHUNK):
+                    hi = min(seg.end, lo + _RECOST_CHUNK)
+                    rec = self.records[lo:hi]
+                    detail = seg.detail_device(lo - seg.first, hi - seg.first, rec, dev)
+                    c, h, st = het_profile_recost(lib, sp, scen, ws, rec, detail, dev)
+                    costs_dev[:, lo:hi], head_dev[:, lo:hi], status_dev[:, lo:hi] = c, h, st
+            costs, headroom, status = costs_dev.cpu().numpy(), head_dev.cpu().numpy(), status_dev.cpu().numpy()
+        t1 = time.perf_counter()
+        usable = (status == 0) & (headroom >= 0)
+        with torch.cuda.device(dev):
+            # an unusable entry at +inf: fmax would skip a NaN, and a plan that does not fit somewhere would look robust
+            masked = torch.from_numpy(np.where(usable, costs, np.inf)).to(dev)
+            best, regret = recost_regret(masked)
+        t2 = time.perf_counter()
+        return Recost(self, costs, best, regret, dev, {'recost_s': t1 - t0, 'regret_s': t2 - t1}, headroom, status)
+
     def records_device(self) -> torch.Tensor:
         """The records (estimate_costs order) on the device, uploaded on first use: what the group passes read."""
         if getattr(self, '_records_dev', None) is None:
@@ -1173,6 +1213,30 @@ def het_recost(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.nda
     return costs
 
 
+def het_profile_recost(lib, s_struct, scenarios, workspace: torch.Tensor, records: np.ndarray, detail: torch.Tensor,
+                       device) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """metis_het_profile_recost of ``records`` (host MetisRecord rows) with their detail rows (device uint8 [n, stride])
+    on the bound space under the scenario problems ``scenarios`` (a ctypes array of MetisProblem bound on the device);
+    returns the device costs, headroom and status [K, n].  Asynchronous on the current stream."""
+    n, K = len(records), len(scenarios)
+    with torch.cuda.device(device):
+        costs = torch.empty((K, n), dtype=torch.float64, device=device)
+        headroom = torch.empty((K, n), dtype=torch.float64, device=device)
+        status = torch.empty((K, n), dtype=torch.uint8, device=device)
+        if n == 0:
+            return costs, headroom, status
+        d_rec = upload(records, device)
+        s = torch.cuda.current_stream(device)
+        rc = lib.metis_het_profile_recost(C.byref(s_struct), C.c_void_p(C.addressof(scenarios)), C.c_int32(K),
+                                          C.c_void_p(d_rec.data_ptr()), C.c_int64(n), C.c_void_p(detail.data_ptr()),
+                                          C.c_int32(detail.shape[1]), C.c_void_p(costs.data_ptr()),
+                                          C.c_void_p(headroom.data_ptr()), C.c_void_p(status.data_ptr()),
+                                          C.c_void_p(workspace.data_ptr()), C.c_int64(workspace.numel()),
+                                          C.c_void_p(s.cuda_stream))
+        native.check(rc, 'metis_het_profile_recost')
+    return costs, headroom, status
+
+
 def recost_regret(costs: torch.Tensor) -> Tuple[np.ndarray, np.ndarray]:
     """metis_recost_regret of the device costs [K, n]: (best [K], regret [n]) on the host."""
     K, n = int(costs.shape[0]), int(costs.shape[1])
@@ -1202,18 +1266,29 @@ def stable_cost_order(records: np.ndarray, cost: np.ndarray, device) -> np.ndarr
 
 
 class Recost:
-    """The candidates of one search re-costed under K bandwidth scenarios (HetSearchResult.recost).
+    """The candidates of one search re-costed under K scenarios: bandwidths (HetSearchResult.recost) or profiles
+    (HetSearchResult.recost_profiles).
 
     ``costs[j, i]`` is candidate i's HeteroCostEstimator.get_cost under scenario j, candidates in estimate_costs order;
-    bit for bit what a fresh search under that scenario's cluster returns for the same candidate.  ``regret[i]`` is
-    max_j (costs[j, i] - best cost of scenario j), absolute and in fp64 (costs may be negative on rough profiles)."""
+    for a bandwidth scenario, bit for bit what a fresh search under that scenario's cluster returns for the same
+    candidate.  ``regret[i]`` is max_j (costs[j, i] - best cost of scenario j), absolute and in fp64 (costs may be
+    negative on rough profiles).
+
+    A profile what-if also has ``headroom`` and ``status`` [K, N] and the ``usable`` mask (status == 0 and headroom >=
+    0).  Its rankings list only the candidates usable under the scenario, and its regret takes an unusable entry as
+    +inf: best_costs[j] is the best usable cost (+inf when none is usable, and such a scenario adds nothing to the
+    regret), and robust(k) lists only the candidates usable in every scenario."""
 
     def __init__(self, candidates, costs: np.ndarray, best_costs: np.ndarray, regret: np.ndarray, device,
-                 timings: Dict[str, float]):
+                 timings: Dict[str, float], headroom: Optional[np.ndarray] = None,
+                 status: Optional[np.ndarray] = None):
         self.candidates = candidates
         self.costs = costs                    # float64 [K, N]
         self.best_costs = best_costs          # float64 [K]: min over the candidates of each scenario (+inf when N == 0)
         self.regret = regret                  # float64 [N]
+        self.headroom = headroom              # float64 [K, N] (profile what-if), else None
+        self.status = status                  # uint8 [K, N]: cost code | memory code << 4 (profile what-if), else None
+        self.usable = None if status is None else (status == 0) & (headroom >= 0)
         self.timings = timings
         self._device = device
         self._orders: Dict[int, np.ndarray] = {}
@@ -1230,10 +1305,16 @@ class Recost:
         return j % K
 
     def order(self, j) -> np.ndarray:
-        """Positions of the candidates in scenario j's ranking: by its cost, ties in estimate_costs order."""
+        """Positions of the candidates in scenario j's ranking: by its cost, ties in estimate_costs order (of a profile
+        what-if, only those usable under scenario j)."""
         j = self._scenario(j)
         if j not in self._orders:
-            self._orders[j] = stable_cost_order(self.candidates.records, self.costs[j], self._device)
+            if self.usable is None:
+                self._orders[j] = stable_cost_order(self.candidates.records, self.costs[j], self._device)
+            else:
+                ok = self.usable[j]
+                pos = stable_cost_order(self.candidates.records, np.where(ok, self.costs[j], np.inf), self._device)
+                self._orders[j] = pos[:int(ok.sum())]
         return self._orders[j]
 
     def _tuples(self, pos: np.ndarray, cost: np.ndarray) -> List[Tuple]:
@@ -1255,11 +1336,13 @@ class Recost:
 
     def robust(self, k: int) -> Tuple[np.ndarray, np.ndarray]:
         """The ``k`` candidates of least regret: (positions in estimate_costs order, their regrets), by ascending regret,
-        ties in estimate_costs order."""
+        ties in estimate_costs order (of a profile what-if, only those usable in every scenario)."""
         if int(k) < 0:
             raise ValueError(f'k must be >= 0, not {k}')
         if self._robust is None:
             self._robust = stable_cost_order(self.candidates.records, self.regret, self._device)
+            if self.usable is not None:
+                self._robust = self._robust[self.usable.all(axis=0)[self._robust]]
         pos = self._robust[:int(k)]
         return pos, self.regret[pos]
 
