@@ -365,6 +365,50 @@ int metis_het_profile_recost(const MetisPlanSpace *space, const MetisProblem *sc
                              void *workspace, int64_t workspace_bytes, void *stream);
 
 /*
+ * Profile-noise what-if: the profile what-if above under seeded samples of the searched profile, drawn on the device,
+ * reduced to per-candidate counts without the K x n arrays leaving the device.  Sample j is search.noisy_profile
+ * (profile, sigma, seed, j): every layer-computes and memory entry and every fb_sync of each key multiplied by its own
+ * factor 1 + s * (2u - 1), u from Philox4x32-10 of (j, index, bs, field << 16 | type << 8 | log2 tp) under the seed
+ * (metis_b200/csrc/metis_noise.cuh).  A chunk of `count` samples, j = first .. first + count - 1, goes through three
+ * calls on one stream:
+ *   draw      metis_het_profile_noise_draw: the chunk's layer_compute, layer_memory, exec_full and fb_sync from the
+ *             base problem's (the searched problem, bound on the device), every other table the base's, each sample's
+ *             tables packed, into the workspace
+ *   evaluate  metis_het_profile_noise_eval, per record range: cost[s * ld + i] (NaN when get_cost raises) and
+ *             usable[s * ld + i] (status == 0 and headroom >= 0, as metis_het_profile_recost) of record i under sample
+ *             first + s
+ *   reduce    metis_het_profile_noise_reduce, once all n records are evaluated: per sample, best_pos[s] / best_cost[s]
+ *             the usable record of lowest cost, ties to the lowest position (-1 / NaN when none is usable); per record,
+ *             the chunk's samples added in order to wins (best_pos == i), near (usable and cost <= best_cost * t),
+ *             usable (count), regret (max of cost - best_cost; +inf once unusable) and sum (costs of usable samples,
+ *             left to right).  The caller zeroes wins, near, usable and sum and sets regret to -inf before the first
+ *             chunk; the results do not depend on the chunk size.
+ */
+typedef struct MetisNoiseSpec {
+    double sigma[3][METIS_MAX_TYPES];  /* [field - 1][device type of the problem]: layer-computes, memory, fb_sync;
+                                          each finite, in [0, 1); 0 leaves the field as it is                      */
+    uint64_t seed;
+    int32_t first;                     /* the chunk's first sample j                                                */
+    int32_t count;                     /* samples in the chunk: 1 <= count, first + count <= 65535                  */
+    uint8_t type_code[METIS_MAX_TYPES];/* 1-based utils.DeviceType position of each device type of the problem     */
+    double near_factor;                /* 1.0 + within: finite, >= 1                                                */
+} MetisNoiseSpec;
+
+/* workspace bytes of one chunk of `count` samples of `base`, or METIS_E_ARG */
+int64_t metis_het_profile_noise_workspace_bytes(const MetisProblem *base, int32_t count);
+int metis_het_profile_noise_draw(const MetisProblem *base, const MetisNoiseSpec *spec, void *workspace,
+                                 int64_t workspace_bytes, void *stream);
+/* records / detail as for metis_het_profile_recost; cost, usable [device] spec->count rows of ld >= n entries */
+int metis_het_profile_noise_eval(const MetisPlanSpace *space, const MetisNoiseSpec *spec, const void *workspace,
+                                 const MetisRecord *records, int64_t n, const uint8_t *detail, int32_t detail_stride,
+                                 double *cost, uint8_t *usable, int64_t ld, void *stream);
+/* cost, usable [device] spec->count x n (ld = n); best_pos, best_cost [device] spec->count; wins, near, usable_count,
+ * regret, sum [device] n */
+int metis_het_profile_noise_reduce(const MetisNoiseSpec *spec, const double *cost, const uint8_t *usable, int64_t n,
+                                   int64_t *best_pos, double *best_cost, int32_t *wins, int32_t *near,
+                                   int32_t *usable_count, double *regret, double *sum, void *stream);
+
+/*
  * metis_homo_cost with the cost terms and the per-stage memory sums (HomoCostEstimator.get_cost returns them as
  * stage_memory, model/cost_estimator.py:121-138).
  *   terms        [device] n x 6 doubles: execution, fb_sync, parameter update, dp, pp, batch generate

@@ -468,6 +468,34 @@ class HetSearchResult(Sequence):
                 for prof in profiles]
         return self.candidates.recost_profiles(scen)
 
+    def profile_noise(self, samples: int, sigma, seed: int = 0, within: float = 0.01) -> 'search.ProfileNoise':
+        """Profile-noise what-if: how often each candidate wins, stays within ``within`` (relative) of the best and
+        fits, over ``samples`` seeded samples of the searched profile drawn on the GPU.  Sample j is
+        ``search.noisy_profile(profile, sigma, seed, j)``: every layer-computes and memory entry and every fb_sync
+        multiplied by its own factor 1 + s * (2u - 1), u uniform in [0, 1) from a counter-based generator, s the
+        field's sigma for the device type (a float, or {field: float or {device type: float}} over 'layer-computes',
+        'memory' and 'fb_sync'; each in [0, 1)).  Each sample is evaluated as recost_profiles evaluates a profile, with
+        every candidate's device groups, strategies and layer partition held fixed; only the per-sample best and the
+        per-candidate counts leave the device.  Every array of the returned search.ProfileNoise equals the numpy
+        reductions of recost_profiles over the samples' dicts, bit for bit; under all-zero sigma every sample is the
+        searched profile.  This is not a search under each sample.  ValueError for samples outside 1 .. 65535, a
+        sigma, seed or within out of range, or an unknown field or device type.  With torch.distributed every rank
+        computes locally: no collective is issued."""
+        from . import search
+        if not isinstance(samples, int) or isinstance(samples, bool) or not 1 <= samples <= search.MAX_NOISE_SAMPLES:
+            raise ValueError(f'samples must be an int in [1, {search.MAX_NOISE_SAMPLES}], not {samples!r}')
+        if not search._real(within) or not math.isfinite(within) or within < 0:
+            raise ValueError(f'within must be a finite number >= 0, not {within!r}')
+        sig = search.noise_sigmas(sigma)
+        seed = search.check_seed(seed)
+        problem = self.candidates.problem
+        table = np.zeros((3, native.METIS_MAX_TYPES))
+        codes = [search.device_type_code(name) for name in problem.type_names]
+        for f, field in enumerate(search.NOISE_FIELDS):
+            for t, name in enumerate(problem.type_names):
+                table[f, t] = search._sigma_of(sig, field, name)
+        return self.candidates.profile_noise(table, codes, seed, samples, float(within))
+
     def best(self) -> Optional[Tuple]:
         """argmin (cost, position): the first entry of the ranked list.  The search kernels reduce it on the device
         (het_finalize_kernel: lowest cost, then lowest ordinal, then lowest step), so no sort is needed for it."""

@@ -119,4 +119,11 @@ int stage_replay_tables(const MetisProblem *problem, void *workspace, int64_t wo
 // The workspace bytes stage_replay_tables needs for `problem`, or METIS_E_ARG.  Defined in metis_search.cu.
 int64_t replay_tables_bytes(const MetisProblem *problem);
 
+// One scenario's packed tables, what make_tables needs (the profile what-ifs, metis_profile.cu and metis_noise.cu)
+struct ScenarioTables {
+    MetisProblem p;
+    BlobLayout lay;
+    const uint8_t *blob;
+};
+
 }  // namespace metis

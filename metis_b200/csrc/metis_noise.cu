@@ -1,0 +1,327 @@
+// Profile-noise what-if of a finished search (include/metis_b200.h, metis_het_profile_noise_*).
+//
+//   key_meta_kernel          each profile key's device type, log2(tp) and bs, from key_index: the Philox counter of a
+//                            value names its key by these
+//   noise_rows_kernel        one thread per (sample, key, layer): the sample's layer_compute and layer_memory entries
+//   noise_keys_kernel        one thread per (sample, key): exec_full (the sum of the sample's layer_compute row) and
+//                            fb_sync.  Every other table of a sample is the base problem's, norm_lc included (only the
+//                            balancer reads it, and no balancer runs here).  All samples share the base key set, num_bs
+//                            and lpad, so one BlobLayout; each sample's tables are packed by pack_tables_kernel
+//                            (stage_replay_tables) and described by a ScenarioTables, as in metis_profile.cu.
+//   het_profile_noise_kernel one thread per costed candidate, the block walking the chunk's samples in step, like
+//                            het_profile_recost_kernel and with its per-candidate body (profile_candidate): cost and the
+//                            usable bit of every (sample, candidate)
+//   noise_min / noise_first  per sample, the lowest cost_order_key of a usable candidate, then the lowest position that
+//                            holds it (group_min_kernel / group_first_kernel's two passes, with a warp's minimum taken
+//                            before its one atomicMin)
+//   noise_accumulate_kernel  one thread per candidate, the chunk's samples in order: noise_accumulate (metis_noise.cuh)
+#include <cuda_runtime.h>
+
+#include <cmath>
+#include <cstdint>
+#include <vector>
+
+#include "../../include/metis_b200.h"
+#include "metis_blob.cuh"
+#include "metis_internal.h"
+#include "metis_noise.cuh"
+#include "metis_query.cuh"
+#include "metis_recost.cuh"
+
+namespace metis {
+
+constexpr int kNoiseThreads = 128;
+constexpr int kReduceThreads = 256;
+constexpr int kMaxSamples = 65535;
+constexpr int kNS = METIS_MAX_STAGES, kNL = METIS_MAX_LAYERS;
+
+static inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
+
+// Where a chunk's pieces sit in the workspace (from its 256-aligned start)
+struct NoiseLayout {
+    int64_t desc, meta, arrays, array_stride, replay, replay_stride, total;
+};
+
+static NoiseLayout noise_layout(const MetisProblem &b, int count, int64_t replay_bytes) {
+    NoiseLayout l;
+    const int64_t K = b.num_keys, row = (int64_t)b.num_keys * b.lpad;
+    l.desc = 0;
+    l.meta = align256((int64_t)count * (int64_t)sizeof(ScenarioTables));
+    l.arrays = l.meta + align256(K * 4);
+    l.array_stride = align256((2 * row + 2 * K) * (int64_t)sizeof(double));
+    l.replay = l.arrays + (int64_t)count * l.array_stride;
+    l.replay_stride = align256(replay_bytes);
+    l.total = l.replay + (int64_t)count * l.replay_stride + 256;
+    return l;
+}
+
+__global__ void key_meta_kernel(const __grid_constant__ MetisProblem b, uint32_t *meta) {
+    const int per_type = b.num_tp * b.num_bs;
+    const int e = blockIdx.x * kReduceThreads + threadIdx.x;
+    if (e >= b.num_types * per_type) return;
+    const int k = b.key_index[e];
+    if (k < 0) return;
+    const int ti = e / per_type, r = e % per_type;
+    meta[k] = pack_key_meta(ti, r / b.num_bs, r % b.num_bs + 1);
+}
+
+__global__ void __launch_bounds__(kReduceThreads)
+noise_rows_kernel(const __grid_constant__ MetisProblem b, const __grid_constant__ MetisNoiseSpec spec,
+                  const uint32_t *__restrict__ meta, uint8_t *arrays, long long array_stride) {
+    const long long row = (long long)b.num_keys * b.lpad;
+    const long long e = (long long)blockIdx.x * kReduceThreads + threadIdx.x;
+    if (e >= row) return;
+    const int s = blockIdx.y;
+    const uint32_t j = (uint32_t)(spec.first + s);
+    double *lc = reinterpret_cast<double *>(arrays + s * array_stride), *lm = lc + row;
+    const uint32_t m = meta[e / b.lpad], l = (uint32_t)(e % b.lpad);
+    lc[e] = noisy_value(b.layer_compute[e], spec.sigma[0], spec.type_code, spec.seed, j, m, kNoiseCompute, l);
+    lm[e] = noisy_value(b.layer_memory[e], spec.sigma[1], spec.type_code, spec.seed, j, m, kNoiseMemory, l);
+}
+
+__global__ void __launch_bounds__(kReduceThreads)
+noise_keys_kernel(const __grid_constant__ MetisProblem b, const __grid_constant__ MetisNoiseSpec spec,
+                  const uint32_t *__restrict__ meta, uint8_t *arrays, long long array_stride) {
+    const int k = blockIdx.x * kReduceThreads + threadIdx.x;
+    if (k >= b.num_keys) return;
+    const int s = blockIdx.y;
+    const long long row = (long long)b.num_keys * b.lpad;
+    double *lc = reinterpret_cast<double *>(arrays + s * array_stride), *ef = lc + 2 * row, *fb = ef + b.num_keys;
+    const uint32_t m = meta[k];
+    ef[k] = spec.sigma[0][m & 0xff] == 0.0 ? b.exec_full[k] : noisy_exec_full(lc + (long long)k * b.lpad, b.lpad);
+    fb[k] = noisy_value(b.fb_sync[k], spec.sigma[2], spec.type_code, spec.seed, (uint32_t)(spec.first + s), m,
+                        kNoiseFbSync, 0);
+}
+
+__global__ void __launch_bounds__(kNoiseThreads)
+het_profile_noise_kernel(const __grid_constant__ MetisPlanSpace sp, const ScenarioTables *__restrict__ scen, int K,
+                         const MetisRecord *__restrict__ records, long long n, const uint8_t *__restrict__ detail,
+                         int stride, double *cost, uint8_t *usable, long long ld) {
+    __shared__ Tables s_T;
+    const long long i = (long long)blockIdx.x * kNoiseThreads + threadIdx.x;
+    Scratch<kNS, kNL> w;
+    RecostEvaluator<kNS, kNL> ev(s_T, w);
+    PlanDesc pd;
+    const bool known = i < n && decode_plan(sp, records[i].ordinal, pd) && pd.S <= kNS;
+    for (int j = 0; j < K; ++j) {
+        __syncthreads();                                      // the previous sample's tables are no longer read
+        if (threadIdx.x == 0) s_T = make_tables(scen[j].p, scen[j].lay, scen[j].blob);
+        __syncthreads();
+        if (i >= n) continue;
+        const size_t at = (size_t)j * ld + i;
+        if (!known) {                                         // not a plan of this space: never a searched candidate
+            cost[at] = (double)NAN;
+            usable[at] = 0;
+            continue;
+        }
+        double c, h;
+        const uint8_t st = profile_candidate(ev, pd, detail + (size_t)i * stride, c, h);
+        cost[at] = c;
+        usable[at] = st == 0 && h >= 0.0 ? 1 : 0;
+    }
+}
+
+__device__ __forceinline__ unsigned long long warp_min(unsigned long long v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long u = __shfl_xor_sync(0xffffffffu, v, o);
+        v = u < v ? u : v;
+    }
+    return v;
+}
+
+__global__ void noise_best_init_kernel(int count, unsigned long long *key, unsigned long long *first) {
+    const int s = blockIdx.x * kReduceThreads + threadIdx.x;
+    if (s >= count) return;
+    key[s] = ~0ULL;
+    first[s] = ~0ULL;
+}
+
+// grid (x: blocks striding over the candidates, y: sample)
+__global__ void __launch_bounds__(kReduceThreads)
+noise_min_kernel(const double *__restrict__ cost, const uint8_t *__restrict__ usable, long long n,
+                 unsigned long long *key) {
+    const size_t row = (size_t)blockIdx.y * n;
+    unsigned long long m = ~0ULL;
+    for (long long i = (long long)blockIdx.x * kReduceThreads + threadIdx.x; i < n;
+         i += (long long)gridDim.x * kReduceThreads)
+        if (usable[row + i]) {
+            const unsigned long long k = cost_order_key(cost[row + i]);
+            m = k < m ? k : m;
+        }
+    m = warp_min(m);
+    if ((threadIdx.x & 31) == 0 && m != ~0ULL) atomicMin(&key[blockIdx.y], m);
+}
+
+__global__ void __launch_bounds__(kReduceThreads)
+noise_first_kernel(const double *__restrict__ cost, const uint8_t *__restrict__ usable, long long n,
+                   const unsigned long long *__restrict__ key, unsigned long long *first) {
+    const size_t row = (size_t)blockIdx.y * n;
+    const unsigned long long want = key[blockIdx.y];
+    unsigned long long m = ~0ULL;
+    for (long long i = (long long)blockIdx.x * kReduceThreads + threadIdx.x; i < n;
+         i += (long long)gridDim.x * kReduceThreads)
+        if (usable[row + i] && cost_order_key(cost[row + i]) == want) {
+            m = (unsigned long long)i;
+            break;                                            // later i of this thread are larger
+        }
+    m = warp_min(m);
+    if ((threadIdx.x & 31) == 0 && m != ~0ULL) atomicMin(&first[blockIdx.y], m);
+}
+
+// the position's own cost (not the key's image, which folds -0.0 into +0.0); -1 / NaN for a sample with no usable
+// candidate
+__global__ void noise_best_finish_kernel(int count, const double *__restrict__ cost, long long n,
+                                         unsigned long long *key, unsigned long long *first) {
+    const int s = blockIdx.x * kReduceThreads + threadIdx.x;
+    if (s >= count) return;
+    const unsigned long long f = first[s];
+    reinterpret_cast<double *>(key)[s] = f == ~0ULL ? (double)NAN : cost[(size_t)s * n + f];
+}
+
+__global__ void __launch_bounds__(kReduceThreads)
+noise_accumulate_kernel(int count, double t, const double *__restrict__ cost, const uint8_t *__restrict__ usable,
+                        long long n, const long long *__restrict__ best_pos, const double *__restrict__ best_cost,
+                        int32_t *wins, int32_t *near, int32_t *usable_count, double *regret, double *sum) {
+    const long long i = (long long)blockIdx.x * kReduceThreads + threadIdx.x;
+    if (i >= n) return;
+    int32_t w = wins[i], nr = near[i], u = usable_count[i];
+    double r = regret[i], sm = sum[i];
+    for (int s = 0; s < count; ++s) {
+        const size_t at = (size_t)s * n + i;
+        noise_accumulate(usable[at] != 0, cost[at], best_pos[s] == i, best_cost[s], t, w, nr, u, r, sm);
+    }
+    wins[i] = w;
+    near[i] = nr;
+    usable_count[i] = u;
+    regret[i] = r;
+    sum[i] = sm;
+}
+
+static unsigned blocks_of(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+
+static const char *check_spec(const MetisNoiseSpec *spec, int num_types) {
+    if (spec->count < 1 || spec->count > kMaxSamples || spec->first < 0 || spec->first > kMaxSamples - spec->count)
+        return "samples out of range (1 <= count, first + count <= 65535)";
+    for (int f = 0; f < 3; ++f)
+        for (int t = 0; t < METIS_MAX_TYPES; ++t) {
+            const double s = spec->sigma[f][t];
+            if (!(s >= 0.0 && s < 1.0)) return "sigma must be finite and in [0, 1)";
+        }
+    for (int t = 0; t < num_types; ++t)
+        if (spec->type_code[t] < 1 || spec->type_code[t] > 6) return "type_code out of range (1 .. 6)";
+    if (!std::isfinite(spec->near_factor) || !(spec->near_factor >= 1.0)) return "near_factor must be finite and >= 1";
+    return nullptr;
+}
+
+static uint8_t *aligned(void *workspace) {
+    return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+}
+
+}  // namespace metis
+
+using namespace metis;
+
+extern "C" {
+
+int64_t metis_het_profile_noise_workspace_bytes(const MetisProblem *base, int32_t count) {
+    if (!base || count < 1 || count > kMaxSamples) return METIS_E_ARG;
+    const int64_t b = replay_tables_bytes(base);
+    if (b < 0) return b;
+    return noise_layout(*base, count, b).total;
+}
+
+int metis_het_profile_noise_draw(const MetisProblem *base, const MetisNoiseSpec *spec, void *workspace,
+                                 int64_t workspace_bytes, void *stream_) {
+    if (!base || !spec || !workspace) return fail_arg("metis_het_profile_noise_draw: NULL argument");
+    if (base->num_types < 1 || base->num_types > METIS_MAX_TYPES)
+        return fail_arg("metis_het_profile_noise_draw: num_types out of range");
+    if (const char *why = check_spec(spec, base->num_types)) return fail_arg(why);
+    const int64_t replay = replay_tables_bytes(base);
+    if (replay < 0) return (int)replay;
+    const NoiseLayout lay = noise_layout(*base, spec->count, replay);
+    if (workspace_bytes < lay.total) return METIS_E_CAPACITY;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    uint8_t *ws = aligned(workspace);
+    uint32_t *meta = reinterpret_cast<uint32_t *>(ws + lay.meta);
+    uint8_t *arrays = ws + lay.arrays;
+    const int count = spec->count;
+    key_meta_kernel<<<blocks_of((long long)base->num_types * base->num_tp * base->num_bs, kReduceThreads),
+                      kReduceThreads, 0, stream>>>(*base, meta);
+    const long long row = (long long)base->num_keys * base->lpad;
+    noise_rows_kernel<<<dim3(blocks_of(row, kReduceThreads), count), kReduceThreads, 0, stream>>>(
+        *base, *spec, meta, arrays, lay.array_stride);
+    noise_keys_kernel<<<dim3(blocks_of(base->num_keys, kReduceThreads), count), kReduceThreads, 0, stream>>>(
+        *base, *spec, meta, arrays, lay.array_stride);
+    std::vector<ScenarioTables> desc((size_t)count);
+    for (int s = 0; s < count; ++s) {
+        ScenarioTables &d = desc[(size_t)s];
+        d.p = *base;
+        const double *lc = reinterpret_cast<const double *>(arrays + (int64_t)s * lay.array_stride);
+        d.p.layer_compute = lc;
+        d.p.layer_memory = lc + row;
+        d.p.exec_full = lc + 2 * row;
+        d.p.fb_sync = lc + 2 * row + base->num_keys;
+        const int rc = stage_replay_tables(&d.p, ws + lay.replay + (int64_t)s * lay.replay_stride, lay.replay_stride,
+                                           stream, d.lay, d.blob);
+        if (rc) return rc;
+    }
+    // pageable source: staged before the call returns, so `desc` may go
+    cudaError_t e = cudaMemcpyAsync(ws + lay.desc, desc.data(), desc.size() * sizeof(ScenarioTables),
+                                    cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return e == cudaSuccess ? METIS_OK : fail_cuda(e, "metis_het_profile_noise_draw");
+}
+
+int metis_het_profile_noise_eval(const MetisPlanSpace *space, const MetisNoiseSpec *spec, const void *workspace,
+                                 const MetisRecord *records, int64_t n, const uint8_t *detail, int32_t detail_stride,
+                                 double *cost, uint8_t *usable, int64_t ld, void *stream_) {
+    if (!space || !spec || !workspace || (n > 0 && (!records || !detail || !cost || !usable)))
+        return fail_arg("metis_het_profile_noise_eval: NULL argument");
+    if (n < 0) return fail_arg("metis_het_profile_noise_eval: negative number of records");
+    if (ld < n) return fail_arg("metis_het_profile_noise_eval: ld < n");
+    if (spec->count < 1 || spec->count > kMaxSamples)
+        return fail_arg("metis_het_profile_noise_eval: count out of range (1 .. 65535)");
+    if (detail_stride < 3 * space->max_stage + 1)
+        return fail_arg("metis_het_profile_noise_eval: detail_stride too small (3 * max_stage + 1)");
+    if (n > 0) {
+        const ScenarioTables *desc = reinterpret_cast<const ScenarioTables *>(aligned(const_cast<void *>(workspace)));
+        het_profile_noise_kernel<<<blocks_of(n, kNoiseThreads), kNoiseThreads, 0, static_cast<cudaStream_t>(stream_)>>>(
+            *space, desc, spec->count, records, n, detail, detail_stride, cost, usable, ld);
+    }
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? METIS_OK : fail_cuda(e, "het_profile_noise_kernel");
+}
+
+int metis_het_profile_noise_reduce(const MetisNoiseSpec *spec, const double *cost, const uint8_t *usable, int64_t n,
+                                   int64_t *best_pos, double *best_cost, int32_t *wins, int32_t *near,
+                                   int32_t *usable_count, double *regret, double *sum, void *stream_) {
+    if (!spec || !best_pos || !best_cost ||
+        (n > 0 && (!cost || !usable || !wins || !near || !usable_count || !regret || !sum)))
+        return fail_arg("metis_het_profile_noise_reduce: NULL argument");
+    if (n < 0) return fail_arg("metis_het_profile_noise_reduce: negative number of records");
+    if (spec->count < 1 || spec->count > kMaxSamples)
+        return fail_arg("metis_het_profile_noise_reduce: count out of range (1 .. 65535)");
+    if (!std::isfinite(spec->near_factor) || !(spec->near_factor >= 1.0))
+        return fail_arg("metis_het_profile_noise_reduce: near_factor must be finite and >= 1");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const int count = spec->count;
+    auto *key = reinterpret_cast<unsigned long long *>(best_cost);
+    auto *first = reinterpret_cast<unsigned long long *>(best_pos);
+    noise_best_init_kernel<<<blocks_of(count, kReduceThreads), kReduceThreads, 0, stream>>>(count, key, first);
+    if (n > 0) {
+        const unsigned bx = blocks_of(n, kReduceThreads) < 64 ? blocks_of(n, kReduceThreads) : 64;
+        noise_min_kernel<<<dim3(bx, count), kReduceThreads, 0, stream>>>(cost, usable, n, key);
+        noise_first_kernel<<<dim3(bx, count), kReduceThreads, 0, stream>>>(cost, usable, n, key, first);
+    }
+    noise_best_finish_kernel<<<blocks_of(count, kReduceThreads), kReduceThreads, 0, stream>>>(count, cost, n, key,
+                                                                                             first);
+    if (n > 0)
+        noise_accumulate_kernel<<<blocks_of(n, kReduceThreads), kReduceThreads, 0, stream>>>(
+            count, spec->near_factor, cost, usable, n, reinterpret_cast<const long long *>(best_pos), best_cost, wins,
+            near, usable_count, regret, sum);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? METIS_OK : fail_cuda(e, "profile noise reduction kernels");
+}
+
+}  // extern "C"

@@ -3,9 +3,9 @@
 //   het_profile_recost_kernel  one thread per costed candidate: the strategies and partition of its detail row and the
 //                              device groups of its plan, held fixed, under every scenario profile in turn.  The block
 //                              walks the scenarios in step: thread 0 binds the block's Tables to scenario j's packed
-//                              blob, then each thread computes get_cost (RecostEvaluator::load + scenario_cost, the
-//                              evaluator of the bandwidth what-if, metis_recost.cuh) and the memory state of every
-//                              stage (PlanEvaluator::stage_memory) under those tables.
+//                              blob, then each thread runs profile_candidate (metis_recost.cuh): get_cost
+//                              (RecostEvaluator::load + scenario_cost, the evaluator of the bandwidth what-if) and the
+//                              memory state of every stage (PlanEvaluator::stage_memory) under those tables.
 //
 // A scenario keeps its own uniform_bw and derived tables: its bandwidths are the searched cluster's, so under the
 // searched profile the kernel computes what the search computed, bit for bit.  Scenarios may differ in key set,
@@ -25,13 +25,6 @@ namespace metis {
 constexpr int kProfileThreads = 128;
 constexpr int kMaxScenarios = 65535;
 constexpr int kPS = METIS_MAX_STAGES, kPL = METIS_MAX_LAYERS;
-
-// One scenario's packed tables, what make_tables needs
-struct ScenarioTables {
-    MetisProblem p;
-    BlobLayout lay;
-    const uint8_t *blob;
-};
 
 static inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
 
@@ -58,18 +51,11 @@ het_profile_recost_kernel(const __grid_constant__ MetisPlanSpace sp, const Scena
             status[at] = (uint8_t)(METIS_FATAL_SCRATCH | METIS_FATAL_SCRATCH << 4);
             continue;
         }
-        const int cost_code = ev.load(pd, detail + (size_t)i * stride) == 0 ? METIS_FATAL_NONE : METIS_FATAL_KEY_EXEC;
-        costs[at] = cost_code == METIS_FATAL_NONE ? ev.scenario_cost() : (double)NAN;
-        int mem_code = METIS_FATAL_NONE;
-        double m = 0.0;
-        for (int s = 0; s < pd.S; ++s) {                      // every stage; lowest first, like the search's headroom
-            double demand, state;
-            const int rc = ev.stage_memory(s, demand, state);
-            if (rc && mem_code == METIS_FATAL_NONE) mem_code = rc;     // the first stage that raises
-            if (s == 0 || state < m) m = state;
-        }
-        headroom[at] = mem_code == METIS_FATAL_NONE ? m : (double)NAN;
-        status[at] = (uint8_t)(cost_code | mem_code << 4);
+        double c, h;
+        const uint8_t st = profile_candidate(ev, pd, detail + (size_t)i * stride, c, h);
+        costs[at] = c;
+        headroom[at] = h;
+        status[at] = st;
     }
 }
 

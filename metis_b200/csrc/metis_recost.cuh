@@ -88,4 +88,25 @@ struct RecostEvaluator : PlanEvaluator<MAXS, MAXL> {
     }
 };
 
+// One candidate of the profile what-ifs (metis_profile.cu, metis_noise.cu) under the tables `ev` is bound to: `cost`
+// get_cost (NaN when it raises), `headroom` the least memory state over every stage, lowest first like the search's
+// headroom (NaN when a stage's demand raises); returns the status cost code | memory code << 4, the memory code that
+// of the first stage that raises.
+template <int MAXS, int MAXL>
+MB_HD uint8_t profile_candidate(RecostEvaluator<MAXS, MAXL> &ev, const PlanDesc &pd, const uint8_t *detail,
+                                double &cost, double &headroom) {
+    const int cost_code = ev.load(pd, detail) == 0 ? METIS_FATAL_NONE : METIS_FATAL_KEY_EXEC;
+    cost = cost_code == METIS_FATAL_NONE ? ev.scenario_cost() : (double)NAN;
+    int mem_code = METIS_FATAL_NONE;
+    double m = 0.0;
+    for (int s = 0; s < pd.S; ++s) {
+        double demand, state;
+        const int rc = ev.stage_memory(s, demand, state);
+        if (rc && mem_code == METIS_FATAL_NONE) mem_code = rc;
+        if (s == 0 || state < m) m = state;
+    }
+    headroom = mem_code == METIS_FATAL_NONE ? m : (double)NAN;
+    return (uint8_t)(cost_code | mem_code << 4);
+}
+
 }  // namespace metis

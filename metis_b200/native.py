@@ -73,6 +73,11 @@ class MetisListing(C.Structure):
                 ('reserved', C.c_int32)]
 
 
+class MetisNoiseSpec(C.Structure):
+    _fields_ = [('sigma', (C.c_double * METIS_MAX_TYPES) * 3), ('seed', C.c_uint64), ('first', C.c_int32),
+                ('count', C.c_int32), ('type_code', C.c_uint8 * METIS_MAX_TYPES), ('near_factor', C.c_double)]
+
+
 class MetisPlanFilter(C.Structure):
     _fields_ = [('min_stages', C.c_int32), ('max_stages', C.c_int32), ('max_repartition', C.c_int32),
                 ('max_tp_code', C.c_int32), ('uniform_tp', C.c_int32), ('flags', C.c_int32),
@@ -108,7 +113,9 @@ SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 
            'metis_list_window', 'metis_het_search_headroom', 'metis_headroom_workspace_bytes', 'metis_headroom_select',
            'metis_headroom_front', 'metis_het_search_outputs', 'metis_het_recost', 'metis_recost_regret_workspace_bytes',
            'metis_recost_regret', 'metis_query_mark', 'metis_query_groups', 'metis_mask_select',
-           'metis_het_profile_recost_workspace_bytes', 'metis_het_profile_recost']
+           'metis_het_profile_recost_workspace_bytes', 'metis_het_profile_recost',
+           'metis_het_profile_noise_workspace_bytes', 'metis_het_profile_noise_draw', 'metis_het_profile_noise_eval',
+           'metis_het_profile_noise_reduce']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -178,6 +185,18 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_het_profile_recost.argtypes = [C.POINTER(MetisPlanSpace), C.c_void_p, C.c_int32, C.c_void_p, C.c_int64,
                                              C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_int64, C.c_void_p]
+    lib.metis_het_profile_noise_workspace_bytes.restype = C.c_int64
+    lib.metis_het_profile_noise_workspace_bytes.argtypes = [C.POINTER(MetisProblem), C.c_int32]
+    lib.metis_het_profile_noise_draw.restype = C.c_int
+    lib.metis_het_profile_noise_draw.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisNoiseSpec), C.c_void_p,
+                                                 C.c_int64, C.c_void_p]
+    lib.metis_het_profile_noise_eval.restype = C.c_int
+    lib.metis_het_profile_noise_eval.argtypes = [C.POINTER(MetisPlanSpace), C.POINTER(MetisNoiseSpec), C.c_void_p,
+                                                 C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                 C.c_int64, C.c_void_p]
+    lib.metis_het_profile_noise_reduce.restype = C.c_int
+    lib.metis_het_profile_noise_reduce.argtypes = [C.POINTER(MetisNoiseSpec)] + [C.c_void_p] * 2 + [C.c_int64] + \
+        [C.c_void_p] * 8
     lib.metis_query_mark.restype = C.c_int
     lib.metis_query_mark.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisPlanFilter),
                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_void_p,

@@ -7,6 +7,7 @@ include/metis_b200.h.  There is no CPU path: without CUDA these functions raise.
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import math
 import time
@@ -705,6 +706,73 @@ class Candidates:
         t2 = time.perf_counter()
         return Recost(self, costs, best, regret, dev, {'recost_s': t1 - t0, 'regret_s': t2 - t1}, headroom, status)
 
+    def profile_noise(self, sigma: np.ndarray, type_code: Sequence[int], seed: int, samples: int,
+                      within: float) -> 'ProfileNoise':
+        """The profile-noise what-if of every candidate over samples 0 .. ``samples`` - 1 of the searched profile
+        (noisy_profile), drawn, evaluated and reduced on the device (metis_het_profile_noise_*).  ``sigma`` [3,
+        METIS_MAX_TYPES] and ``type_code`` are per device type of the searched problem.  The samples go in chunks sized
+        by _NOISE_BUDGET_BYTES; each chunk is drawn and packed once, then evaluated segment by segment, _RECOST_CHUNK
+        records per launch (a window replays its detail rows once per chunk), then reduced.  Only the per-sample best
+        and the per-candidate counts come back.  timings: ``noise_s`` the whole call, ``chunks`` how many."""
+        t0 = time.perf_counter()
+        dev = _require_cuda(self.device)
+        n = len(self.records)
+        spec = native.MetisNoiseSpec()
+        for f in range(3):
+            for t in range(native.METIS_MAX_TYPES):
+                spec.sigma[f][t] = float(sigma[f][t])
+        for t, code in enumerate(type_code):
+            spec.type_code[t] = int(code)
+        spec.seed = int(seed)
+        spec.near_factor = 1.0 + float(within)
+        with torch.cuda.device(dev):
+            lib, p, _sp, _ws, _keep = bind_problem(self.problem, dev, workspace=False)
+            one = int(lib.metis_het_profile_noise_workspace_bytes(C.byref(p), 1))
+            native.check(min(one, 0), 'metis_het_profile_noise_workspace_bytes')
+            per = int(lib.metis_het_profile_noise_workspace_bytes(C.byref(p), 2)) - one
+            chunk = int(max(1, min(samples, (_NOISE_BUDGET_BYTES - one + per) // (per + 9 * max(n, 1)))))
+            ws = torch.empty(int(lib.metis_het_profile_noise_workspace_bytes(C.byref(p), chunk)), dtype=torch.uint8,
+                             device=dev)
+            cost = torch.empty((chunk, max(n, 1)), dtype=torch.float64, device=dev)
+            usable = torch.empty((chunk, max(n, 1)), dtype=torch.uint8, device=dev)
+            best_pos = torch.empty(samples, dtype=torch.int64, device=dev)
+            best_cost = torch.empty(samples, dtype=torch.float64, device=dev)
+            wins, near, count = (torch.zeros(max(n, 1), dtype=torch.int32, device=dev) for _ in range(3))
+            regret = torch.full((max(n, 1),), -math.inf, dtype=torch.float64, device=dev)
+            total = torch.zeros(max(n, 1), dtype=torch.float64, device=dev)
+            s = torch.cuda.current_stream(dev)
+            ptr = lambda t, off=0: C.c_void_p(t.data_ptr() + off)              # noqa: E731
+            for first in range(0, samples, chunk):
+                spec.first, spec.count = first, min(chunk, samples - first)
+                native.check(lib.metis_het_profile_noise_draw(C.byref(p), C.byref(spec), ptr(ws), C.c_int64(ws.numel()),
+                                                              C.c_void_p(s.cuda_stream)), 'metis_het_profile_noise_draw')
+                for seg in self.segments:
+                    if seg.first == seg.end:
+                        continue
+                    _lib, _p, sp, _w, _d, _k = seg.bind()
+                    for lo in range(seg.first, seg.end, _RECOST_CHUNK):
+                        hi = min(seg.end, lo + _RECOST_CHUNK)
+                        rec = self.records[lo:hi]
+                        detail = seg.detail_device(lo - seg.first, hi - seg.first, rec, dev)
+                        d_rec = upload(rec, dev)
+                        native.check(lib.metis_het_profile_noise_eval(
+                            C.byref(sp), C.byref(spec), ptr(ws), ptr(d_rec), C.c_int64(hi - lo), ptr(detail),
+                            C.c_int32(detail.shape[1]), ptr(cost, 8 * lo), ptr(usable, lo), C.c_int64(n),
+                            C.c_void_p(s.cuda_stream)), 'metis_het_profile_noise_eval')
+                native.check(lib.metis_het_profile_noise_reduce(
+                    C.byref(spec), ptr(cost), ptr(usable), C.c_int64(n), ptr(best_pos, 8 * first),
+                    ptr(best_cost, 8 * first), ptr(wins), ptr(near), ptr(count), ptr(regret), ptr(total),
+                    C.c_void_p(s.cuda_stream)), 'metis_het_profile_noise_reduce')
+            out = [t.cpu().numpy() for t in (best_pos, best_cost, wins, near, count, regret, total)]
+        best_pos, best_cost, wins, near, count, regret, total = out
+        wins, near, count, regret, total = (a[:n] for a in (wins, near, count, regret, total))
+        with np.errstate(invalid='ignore', divide='ignore'):
+            mean = np.where(count > 0, total / np.maximum(count, 1), np.nan)
+        t1 = time.perf_counter()
+        return ProfileNoise(self, best_pos, best_cost, wins.astype(np.int64), near.astype(np.int64),
+                            count.astype(np.int64), regret, mean,
+                            {'noise_s': t1 - t0, 'chunks': -(-samples // chunk), 'chunk': chunk})
+
     def records_device(self) -> torch.Tensor:
         """The records (estimate_costs order) on the device, uploaded on first use: what the group passes read."""
         if getattr(self, '_records_dev', None) is None:
@@ -1345,6 +1413,182 @@ class Recost:
                 self._robust = self._robust[self.usable.all(axis=0)[self._robust]]
         pos = self._robust[:int(k)]
         return pos, self.regret[pos]
+
+
+# ---------------------------------------------------------------------------------------------
+# profile-noise what-if: seeded samples of the searched profile (noisy_profile), evaluated and reduced on the device
+# ---------------------------------------------------------------------------------------------
+NOISE_FIELDS = ('layer-computes', 'memory', 'fb_sync')       # field codes 1, 2, 3 of the Philox counter
+MAX_NOISE_SAMPLES = 65535
+_NOISE_BUDGET_BYTES = 1 << 30             # device memory of one chunk of samples: workspace, costs and usable bits
+_M32 = 0xFFFFFFFF
+
+
+def philox4x32_10(counter: Sequence[int], key: Sequence[int]) -> Tuple[int, int, int, int]:
+    """Philox4x32-10 (Salmon et al., SC'11, the Random123 constants) of four 32-bit counter words under two key words."""
+    c0, c1, c2, c3 = (int(v) & _M32 for v in counter)
+    k0, k1 = (int(v) & _M32 for v in key)
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + 0x9E3779B9) & _M32, (k1 + 0xBB67AE85) & _M32
+        p0, p1 = 0xD2511F53 * c0, 0xCD9E8D57 * c2
+        c0, c1, c2, c3 = ((p1 >> 32) ^ c1 ^ k0) & _M32, p1 & _M32, ((p0 >> 32) ^ c3 ^ k1) & _M32, p0 & _M32
+    return c0, c1, c2, c3
+
+
+def noise_factor(s: float, seed: int, j: int, index: int, bs: int, field: int, type_code: int, tpl: int) -> float:
+    """The factor 1 + s * (2u - 1) of one value of sample j (metis_noise.cuh's noise_factor)."""
+    r0, r1, _, _ = philox4x32_10((j, index, bs, field << 16 | type_code << 8 | tpl), (seed & _M32, seed >> 32))
+    u = ((r0 << 32 | r1) >> 11) * 2.0 ** -53
+    return 1.0 + s * (2.0 * u - 1.0)
+
+
+def _real(v) -> bool:
+    return isinstance(v, (int, float)) and not isinstance(v, bool)
+
+
+def _sigma_value(v, where: str) -> float:
+    if not _real(v) or not math.isfinite(v) or not 0.0 <= v < 1.0:
+        raise ValueError(f'sigma {where}: must be a finite number in [0, 1), not {v!r}')
+    return float(v)
+
+
+def noise_sigmas(sigma) -> Dict[str, Tuple[float, Dict[str, float]]]:
+    """``sigma`` (a float for every field and device type, or {field: float or {device type: float}}, fields of
+    NOISE_FIELDS, device types named as in utils.DeviceType) as {field: (sigma of a type not named, {type: sigma})}.
+    ValueError for an unknown field or device type, or a sigma that is not finite or outside [0, 1)."""
+    from .utils import DeviceType
+    if not isinstance(sigma, dict):
+        s = _sigma_value(sigma, 'for every field')
+        return {f: (s, {}) for f in NOISE_FIELDS}
+    out = {f: (0.0, {}) for f in NOISE_FIELDS}
+    for field, v in sigma.items():
+        if field not in NOISE_FIELDS:
+            raise ValueError(f'sigma: unknown field {field!r} (one of {", ".join(NOISE_FIELDS)})')
+        if isinstance(v, dict):
+            per = {}
+            for name, s in v.items():
+                if name not in DeviceType.__members__:
+                    raise ValueError(f'sigma {field!r}: unknown device type {name!r}')
+                per[name] = _sigma_value(s, f'{field!r} {name}')
+            out[field] = (0.0, per)
+        else:
+            out[field] = (_sigma_value(v, repr(field)), {})
+    return out
+
+
+def _sigma_of(sig, field: str, type_name: str) -> float:
+    default, per = sig[field]
+    return per.get(type_name, default)
+
+
+def check_seed(seed) -> int:
+    if not isinstance(seed, int) or isinstance(seed, bool) or not 0 <= seed < 2 ** 64:
+        raise ValueError(f'seed must be an int in [0, 2^64), not {seed!r}')
+    return seed
+
+
+def device_type_code(name: str) -> int:
+    """The 1-based position of device type ``name`` in utils.DeviceType (A100 = 1 ... B200 = 6)."""
+    from .utils import DeviceType
+    names = list(DeviceType.__members__)
+    if name not in names:
+        raise ValueError(f'unknown device type {name!r}')
+    return names.index(name) + 1
+
+
+def noisy_profile(profile: Dict, sigma, seed: int, j: int) -> Dict:
+    """Sample ``j`` of ``profile`` (a dict like ProfileDataLoader.load_profile_data_all()[0]) under ``sigma`` and
+    ``seed``: a deep copy whose every ``time.layer-computes`` entry (field 1), ``memory`` entry (field 2) and
+    ``time.fb_sync`` (field 3) of every DeviceType.<T> / tp<t>_bs<b> entry is multiplied by its own factor
+    f = 1.0 + s * (2.0 * u - 1.0), s the field's sigma for T (noise_sigmas), u = ((r0 << 32 | r1) >> 11) * 2**-53 and
+    (r0, r1, r2, r3) = Philox4x32-10 of the counter (j, index in the list (0 for fb_sync), b,
+    field << 16 | type << 8 | log2(t)) under the key (seed & 0xffffffff, seed >> 32), type the 1-based position of T in
+    utils.DeviceType.  Every operation is one IEEE double operation.  A field whose sigma is 0 is left as it is (ints
+    stay ints); the 'model' section is never touched.  This is the definition of the samples of
+    HetSearchResult.profile_noise."""
+    sig = noise_sigmas(sigma)
+    seed = check_seed(seed)
+    if not isinstance(j, int) or isinstance(j, bool) or not 0 <= j <= _M32:
+        raise ValueError(f'sample index must be an int in [0, 2^32), not {j!r}')
+    out = copy.deepcopy(profile)
+    for entry_name, entries in out.items():
+        if not entry_name.startswith('DeviceType.'):
+            continue
+        name = entry_name[len('DeviceType.'):]
+        s = [_sigma_of(sig, f, name) for f in NOISE_FIELDS]
+        if not any(s):
+            continue
+        code = device_type_code(name)
+        for key, entry in entries.items():
+            t, b = int(key[2:].split('_bs')[0]), int(key.split('_bs')[1])
+            tpl = t.bit_length() - 1
+            tm = entry['time']
+            if s[0]:
+                tm['layer-computes'] = [v * noise_factor(s[0], seed, j, i, b, 1, code, tpl)
+                                        for i, v in enumerate(tm['layer-computes'])]
+            if s[1]:
+                entry['memory'] = [v * noise_factor(s[1], seed, j, i, b, 2, code, tpl)
+                                   for i, v in enumerate(entry['memory'])]
+            if s[2] and _real(tm.get('fb_sync')):
+                tm['fb_sync'] = tm['fb_sync'] * noise_factor(s[2], seed, j, 0, b, 3, code, tpl)
+    return out
+
+
+class ProfileNoise:
+    """The profile-noise what-if of one search (HetSearchResult.profile_noise): every candidate, with its device groups,
+    strategies and layer partition held fixed, under K seeded samples of the searched profile (noisy_profile).  With
+    c[j, i], usable[j, i] what recost_profiles gives candidate i under sample j:
+
+      best_pos[j], best_cost[j]  the usable candidate of lowest cost, ties to the lowest position (-1, NaN: none)
+      wins[i]                    samples whose best_pos is i
+      usable[i]                  samples in which candidate i is usable
+      near[i]                    samples in which it is usable and c[j, i] <= best_cost[j] * (1.0 + within)
+      regret[i]                  max_j (c[j, i] - best_cost[j]); +inf if it is unusable in any sample
+      mean[i]                    its costs over the samples where it is usable, added in sample order, / usable[i]
+                                 (NaN when usable[i] is 0)
+
+    Candidates are in estimate_costs order.  Nothing here is a search under a sample: a search would re-run the
+    strategy chain and the balancer and pick other partitions."""
+
+    _DESCENDING = ('wins', 'near')
+    _ASCENDING = ('regret', 'mean')
+
+    def __init__(self, candidates, best_pos, best_cost, wins, near, usable, regret, mean, timings):
+        self.candidates = candidates
+        self.best_pos = best_pos              # int64 [K]
+        self.best_cost = best_cost            # float64 [K]
+        self.wins = wins                      # int64 [N]
+        self.near = near                      # int64 [N]
+        self.usable = usable                  # int64 [N]
+        self.regret = regret                  # float64 [N]
+        self.mean = mean                      # float64 [N]
+        self.timings = timings
+
+    def __len__(self) -> int:
+        return len(self.best_pos)
+
+    def order(self, by: str) -> np.ndarray:
+        """Positions of the candidates by statistic ``by``: wins or near descending, regret or mean ascending (NaN
+        last), ties by the searched cost, then the position."""
+        if by in self._DESCENDING:
+            key = -getattr(self, by)
+        elif by in self._ASCENDING:
+            key = getattr(self, by)
+        else:
+            raise ValueError(f'by must be one of {self._DESCENDING + self._ASCENDING}, not {by!r}')
+        n = len(self.wins)
+        return np.lexsort((np.arange(n), self.candidates.records['cost'][:n], key))
+
+    def ranked(self, by: str, k: Optional[int] = None) -> List[Tuple]:
+        """The first ``k`` (default: all) candidates by ``by`` (order) as the reference's 7-tuples, slot 6 the searched
+        cost.  A ranking of the searched candidates, not a search under the samples."""
+        pos = self.order(by)
+        if k is not None:
+            if int(k) < 0:
+                raise ValueError(f'k must be >= 0, not {k}')
+            pos = pos[:int(k)]
+        return self.candidates.tuples(pos)
 
 
 def materialize(records: np.ndarray, detail: np.ndarray, space: flatten.FlatPlanSpace,
