@@ -126,4 +126,51 @@ struct ScenarioTables {
     const uint8_t *blob;
 };
 
+// Packs the tables of problems[0 .. K) (stage_replay_tables), problem j's at `blobs` + the sum of
+// align256(replay_tables_bytes(problems[i])) for i < j, then writes their K descriptors to `desc` with one
+// host-to-device copy.  Returns METIS_OK or stage_replay_tables' error code; launch and copy errors are left for
+// cudaGetLastError.  Defined in metis_profile.cu.
+int stage_scenarios(const MetisProblem *problems, int K, ScenarioTables *desc, uint8_t *blobs, cudaStream_t stream);
+
+// What het_profile_kernel stores for candidate i of n under scenario j: `unknown` for a record that is no plan of the
+// space, else `store` with profile_candidate's cost, headroom and status (metis_recost.cuh).
+struct ProfileOut {                   // metis_het_profile_recost: all three, at j * n + i
+    double *cost, *headroom;
+    uint8_t *status;
+    __device__ void unknown(int j, long long i, long long n) const {
+        const size_t at = (size_t)j * n + i;
+        cost[at] = headroom[at] = (double)NAN;
+        status[at] = (uint8_t)(METIS_FATAL_SCRATCH | METIS_FATAL_SCRATCH << 4);
+    }
+    __device__ void store(int j, long long i, long long n, double c, double h, uint8_t st) const {
+        const size_t at = (size_t)j * n + i;
+        cost[at] = c;
+        headroom[at] = h;
+        status[at] = st;
+    }
+};
+
+struct NoiseOut {                     // metis_het_profile_noise_eval: cost and the usable byte, at j * ld + i
+    double *cost;
+    uint8_t *usable;
+    long long ld;
+    __device__ void unknown(int j, long long i, long long) const {
+        const size_t at = (size_t)j * ld + i;
+        cost[at] = (double)NAN;
+        usable[at] = 0;
+    }
+    __device__ void store(int j, long long i, long long, double c, double h, uint8_t st) const {
+        const size_t at = (size_t)j * ld + i;
+        cost[at] = c;
+        usable[at] = st == 0 && h >= 0.0 ? 1 : 0;
+    }
+};
+
+// Launches het_profile_kernel (metis_profile.cu) on `stream` when n > 0: one thread per record of records[0 .. n)
+// (detail row at detail + i * stride), the block walking the K scenarios of `scen` in step.  Launch errors are left
+// for cudaGetLastError.
+template <class Out>
+void launch_profile_kernel(const MetisPlanSpace &sp, const ScenarioTables *scen, int K, const MetisRecord *records,
+                           int64_t n, const uint8_t *detail, int stride, const Out &out, cudaStream_t stream);
+
 }  // namespace metis

@@ -35,8 +35,6 @@ struct Layout {
            irec = 0, ipool = 0, partials = 0, bytes = 0;
 };
 
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 int64_t scan_blocks(int64_t n) { return (n + kScanTile - 1) / kScanTile; }
 
 // the counting table, the first shape and first composition of every stage count, and the workspace layout

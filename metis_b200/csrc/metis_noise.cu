@@ -6,11 +6,10 @@
 //   noise_keys_kernel        one thread per (sample, key): exec_full (the sum of the sample's layer_compute row) and
 //                            fb_sync.  Every other table of a sample is the base problem's, norm_lc included (only the
 //                            balancer reads it, and no balancer runs here).  All samples share the base key set, num_bs
-//                            and lpad, so one BlobLayout; each sample's tables are packed by pack_tables_kernel
-//                            (stage_replay_tables) and described by a ScenarioTables, as in metis_profile.cu.
-//   het_profile_noise_kernel one thread per costed candidate, the block walking the chunk's samples in step, like
-//                            het_profile_recost_kernel and with its per-candidate body (profile_candidate): cost and the
-//                            usable bit of every (sample, candidate)
+//                            and lpad, so one BlobLayout; stage_scenarios (metis_profile.cu) packs each sample's
+//                            tables and writes their descriptors.
+//   het_profile_kernel       metis_profile.cu's kernel of the profile what-if, launched with NoiseOut: cost and the
+//                            usable byte of every (sample, candidate)
 //   noise_min / noise_first  per sample, the lowest cost_order_key of a usable candidate, then the lowest position that
 //                            holds it (group_min_kernel / group_first_kernel's two passes, with a warp's minimum taken
 //                            before its one atomicMin)
@@ -26,16 +25,11 @@
 #include "metis_internal.h"
 #include "metis_noise.cuh"
 #include "metis_query.cuh"
-#include "metis_recost.cuh"
 
 namespace metis {
 
-constexpr int kNoiseThreads = 128;
 constexpr int kReduceThreads = 256;
 constexpr int kMaxSamples = 65535;
-constexpr int kNS = METIS_MAX_STAGES, kNL = METIS_MAX_LAYERS;
-
-static inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
 
 // Where a chunk's pieces sit in the workspace (from its 256-aligned start)
 struct NoiseLayout {
@@ -91,34 +85,6 @@ noise_keys_kernel(const __grid_constant__ MetisProblem b, const __grid_constant_
     ef[k] = spec.sigma[0][m & 0xff] == 0.0 ? b.exec_full[k] : noisy_exec_full(lc + (long long)k * b.lpad, b.lpad);
     fb[k] = noisy_value(b.fb_sync[k], spec.sigma[2], spec.type_code, spec.seed, (uint32_t)(spec.first + s), m,
                         kNoiseFbSync, 0);
-}
-
-__global__ void __launch_bounds__(kNoiseThreads)
-het_profile_noise_kernel(const __grid_constant__ MetisPlanSpace sp, const ScenarioTables *__restrict__ scen, int K,
-                         const MetisRecord *__restrict__ records, long long n, const uint8_t *__restrict__ detail,
-                         int stride, double *cost, uint8_t *usable, long long ld) {
-    __shared__ Tables s_T;
-    const long long i = (long long)blockIdx.x * kNoiseThreads + threadIdx.x;
-    Scratch<kNS, kNL> w;
-    RecostEvaluator<kNS, kNL> ev(s_T, w);
-    PlanDesc pd;
-    const bool known = i < n && decode_plan(sp, records[i].ordinal, pd) && pd.S <= kNS;
-    for (int j = 0; j < K; ++j) {
-        __syncthreads();                                      // the previous sample's tables are no longer read
-        if (threadIdx.x == 0) s_T = make_tables(scen[j].p, scen[j].lay, scen[j].blob);
-        __syncthreads();
-        if (i >= n) continue;
-        const size_t at = (size_t)j * ld + i;
-        if (!known) {                                         // not a plan of this space: never a searched candidate
-            cost[at] = (double)NAN;
-            usable[at] = 0;
-            continue;
-        }
-        double c, h;
-        const uint8_t st = profile_candidate(ev, pd, detail + (size_t)i * stride, c, h);
-        cost[at] = c;
-        usable[at] = st == 0 && h >= 0.0 ? 1 : 0;
-    }
 }
 
 __device__ __forceinline__ unsigned long long warp_min(unsigned long long v) {
@@ -214,10 +180,6 @@ static const char *check_spec(const MetisNoiseSpec *spec, int num_types) {
     return nullptr;
 }
 
-static uint8_t *aligned(void *workspace) {
-    return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-}
-
 }  // namespace metis
 
 using namespace metis;
@@ -242,7 +204,7 @@ int metis_het_profile_noise_draw(const MetisProblem *base, const MetisNoiseSpec 
     const NoiseLayout lay = noise_layout(*base, spec->count, replay);
     if (workspace_bytes < lay.total) return METIS_E_CAPACITY;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    uint8_t *ws = aligned(workspace);
+    uint8_t *ws = align_workspace(workspace);
     uint32_t *meta = reinterpret_cast<uint32_t *>(ws + lay.meta);
     uint8_t *arrays = ws + lay.arrays;
     const int count = spec->count;
@@ -253,23 +215,18 @@ int metis_het_profile_noise_draw(const MetisProblem *base, const MetisNoiseSpec 
         *base, *spec, meta, arrays, lay.array_stride);
     noise_keys_kernel<<<dim3(blocks_of(base->num_keys, kReduceThreads), count), kReduceThreads, 0, stream>>>(
         *base, *spec, meta, arrays, lay.array_stride);
-    std::vector<ScenarioTables> desc((size_t)count);
+    std::vector<MetisProblem> samples((size_t)count, *base);
     for (int s = 0; s < count; ++s) {
-        ScenarioTables &d = desc[(size_t)s];
-        d.p = *base;
         const double *lc = reinterpret_cast<const double *>(arrays + (int64_t)s * lay.array_stride);
-        d.p.layer_compute = lc;
-        d.p.layer_memory = lc + row;
-        d.p.exec_full = lc + 2 * row;
-        d.p.fb_sync = lc + 2 * row + base->num_keys;
-        const int rc = stage_replay_tables(&d.p, ws + lay.replay + (int64_t)s * lay.replay_stride, lay.replay_stride,
-                                           stream, d.lay, d.blob);
-        if (rc) return rc;
+        samples[(size_t)s].layer_compute = lc;
+        samples[(size_t)s].layer_memory = lc + row;
+        samples[(size_t)s].exec_full = lc + 2 * row;
+        samples[(size_t)s].fb_sync = lc + 2 * row + base->num_keys;
     }
-    // pageable source: staged before the call returns, so `desc` may go
-    cudaError_t e = cudaMemcpyAsync(ws + lay.desc, desc.data(), desc.size() * sizeof(ScenarioTables),
-                                    cudaMemcpyHostToDevice, stream);
-    if (e == cudaSuccess) e = cudaGetLastError();
+    const int rc = stage_scenarios(samples.data(), count, reinterpret_cast<ScenarioTables *>(ws + lay.desc),
+                                   ws + lay.replay, stream);
+    if (rc) return rc;
+    const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? METIS_OK : fail_cuda(e, "metis_het_profile_noise_draw");
 }
 
@@ -284,13 +241,11 @@ int metis_het_profile_noise_eval(const MetisPlanSpace *space, const MetisNoiseSp
         return fail_arg("metis_het_profile_noise_eval: count out of range (1 .. 65535)");
     if (detail_stride < 3 * space->max_stage + 1)
         return fail_arg("metis_het_profile_noise_eval: detail_stride too small (3 * max_stage + 1)");
-    if (n > 0) {
-        const ScenarioTables *desc = reinterpret_cast<const ScenarioTables *>(aligned(const_cast<void *>(workspace)));
-        het_profile_noise_kernel<<<blocks_of(n, kNoiseThreads), kNoiseThreads, 0, static_cast<cudaStream_t>(stream_)>>>(
-            *space, desc, spec->count, records, n, detail, detail_stride, cost, usable, ld);
-    }
+    const ScenarioTables *desc = reinterpret_cast<const ScenarioTables *>(align_workspace(const_cast<void *>(workspace)));
+    launch_profile_kernel(*space, desc, spec->count, records, n, detail, detail_stride, NoiseOut{cost, usable, ld},
+                          static_cast<cudaStream_t>(stream_));
     const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? METIS_OK : fail_cuda(e, "het_profile_noise_kernel");
+    return e == cudaSuccess ? METIS_OK : fail_cuda(e, "het_profile_kernel");
 }
 
 int metis_het_profile_noise_reduce(const MetisNoiseSpec *spec, const double *cost, const uint8_t *usable, int64_t n,

@@ -190,13 +190,13 @@ int metis_sort_records(MetisRecord *records, int64_t n, int32_t mode, uint32_t *
     const int rc = rank_grid(&blocks);
     if (rc) return rc;
     if ((int64_t)blocks * kRankWarps > kRankMaxWarps) blocks = (int)(kRankMaxWarps / kRankWarps);
-    uint8_t *p = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+    uint8_t *p = align_workspace(workspace);
     RankArgs q;
     q.a = reinterpret_cast<uint4 *>(records);
     q.b = reinterpret_cast<uint4 *>(p);            p += n * 16;
     q.ia = reinterpret_cast<uint32_t *>(p);        p += n * 4;
     q.ib = reinterpret_cast<uint32_t *>(p);        p += n * 4;
-    p = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(p) + 255) & ~(uintptr_t)255);
+    p = align_workspace(p);
     q.hist = reinterpret_cast<unsigned int *>(p);  p += 256 * (int64_t)blocks * kRankWarps * 4;
     q.bintot = reinterpret_cast<unsigned int *>(p);
     q.n = n;

@@ -156,7 +156,7 @@ int metis_recost_regret(const double *costs, int32_t num_scenarios, int64_t n, d
     if (!best || !workspace || (n > 0 && (!costs || !regret))) return fail_arg("metis_recost_regret: NULL argument");
     if (workspace_bytes < metis_recost_regret_workspace_bytes(num_scenarios, n)) return METIS_E_CAPACITY;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    double *tile_min = reinterpret_cast<double *>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+    double *tile_min = reinterpret_cast<double *>(align_workspace(workspace));
     const long long nt = regret_tiles(n);                     // one empty tile when n == 0: best[j] = +inf
     tile_min_kernel<<<dim3((unsigned)nt, (unsigned)num_scenarios), kRegThreads, 0, stream>>>(costs, n, tile_min);
     best_kernel<<<(unsigned)num_scenarios, kRegScan, 0, stream>>>(tile_min, nt, best);

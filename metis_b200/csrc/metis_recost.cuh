@@ -20,8 +20,9 @@ struct RecostEvaluator : PlanEvaluator<MAXS, MAXL> {
     double exec, fb_sync, max_upd, bg;
 
     // For the bandwidth what-if (metis_het_recost), `t` must read its bandwidths through the general path
-    // (t.p.uniform_bw == 0): its bw_first / bw_min hold the scenario when scenario_cost is called.  The profile what-if
-    // (metis_profile.cu) binds `t` to a whole scenario's tables, derived bandwidth tables included.
+    // (t.p.uniform_bw == 0): its bw_first / bw_min hold the scenario when scenario_cost is called.  The profile
+    // what-ifs (het_profile_kernel, metis_profile.cu) bind `t` to a whole scenario's tables, derived bandwidth tables
+    // included.
     MB_HD RecostEvaluator(const Tables &t, Scratch<MAXS, MAXL> &s) : Base(t, s), nstage(0), exec(0), fb_sync(0), max_upd(0), bg(0) {}
 
     // The candidate: plan `plan` with the strategies and partition of its detail row (dp codes[S], tp codes[S],
@@ -88,10 +89,10 @@ struct RecostEvaluator : PlanEvaluator<MAXS, MAXL> {
     }
 };
 
-// One candidate of the profile what-ifs (metis_profile.cu, metis_noise.cu) under the tables `ev` is bound to: `cost`
-// get_cost (NaN when it raises), `headroom` the least memory state over every stage, lowest first like the search's
-// headroom (NaN when a stage's demand raises); returns the status cost code | memory code << 4, the memory code that
-// of the first stage that raises.
+// One candidate of the profile what-ifs (het_profile_kernel, metis_profile.cu) under the tables `ev` is bound to:
+// `cost` get_cost (NaN when it raises), `headroom` the least memory state over every stage, lowest first like the
+// search's headroom (NaN when a stage's demand raises); returns the status cost code | memory code << 4, the memory
+// code that of the first stage that raises.
 template <int MAXS, int MAXL>
 MB_HD uint8_t profile_candidate(RecostEvaluator<MAXS, MAXL> &ev, const PlanDesc &pd, const uint8_t *detail,
                                 double &cost, double &headroom) {

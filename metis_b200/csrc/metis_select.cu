@@ -204,10 +204,8 @@ struct SelectWorkspace {
 
 static long long num_tiles(int64_t n) { return n > 0 ? (n + kTile - 1) / kTile : 1; }
 
-static int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
 static SelectWorkspace carve_select(void *ws, int64_t n) {
-    uint8_t *p = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
+    uint8_t *p = align_workspace(ws);
     const long long nt = num_tiles(n);
     SelectWorkspace w;
     w.tile_count = reinterpret_cast<unsigned long long *>(p); p += align256(nt * 8);

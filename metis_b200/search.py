@@ -36,6 +36,11 @@ def upload(a: np.ndarray, device) -> torch.Tensor:
     return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).to(device)
 
 
+def _ptr(t: torch.Tensor, offset: int = 0) -> C.c_void_p:
+    """The device address ``offset`` bytes into ``t``."""
+    return C.c_void_p(t.data_ptr() + offset)
+
+
 def bind_problem(problem: flatten.FlatProblem, device, space: Optional[flatten.FlatPlanSpace] = None,
                  rows: Optional[torch.Tensor] = None, workspace: bool = True):
     """``problem``'s tables (and ``space``'s blocks and batches, with ``rows``, its device-group rows on ``device``)
@@ -649,18 +654,18 @@ class Candidates:
         the host, ``regret_s`` the regret kernels and their copy."""
         t0 = time.perf_counter()
         dev = _require_cuda(self.device)
+        K = len(bandwidths)
         with torch.cuda.device(dev):
             bw = torch.from_numpy(np.ascontiguousarray(bandwidths, dtype=np.float64)).to(dev)
-            costs_dev = torch.empty((len(bandwidths), len(self.records)), dtype=torch.float64, device=dev)
-            for seg in self.segments:
-                if seg.first == seg.end:                      # nothing to replay: a window is not reloaded for it
-                    continue
-                lib, p, sp, ws, _dev, _keep = seg.bind()
-                for lo in range(seg.first, seg.end, _RECOST_CHUNK):
-                    hi = min(seg.end, lo + _RECOST_CHUNK)
-                    rec = self.records[lo:hi]
-                    detail = seg.detail_device(lo - seg.first, hi - seg.first, rec, dev)
-                    costs_dev[:, lo:hi] = het_recost(lib, p, sp, ws, rec, detail, bw, dev)
+            costs_dev = torch.empty((K, len(self.records)), dtype=torch.float64, device=dev)
+            s = torch.cuda.current_stream(dev)
+            for (lib, p, sp, ws, _dev, _keep), lo, hi, rec, detail in self._replay_chunks(dev):
+                c = torch.empty((K, hi - lo), dtype=torch.float64, device=dev)
+                native.check(lib.metis_het_recost(
+                    C.byref(p), C.byref(sp), _ptr(rec), C.c_int64(hi - lo), _ptr(detail), C.c_int32(detail.shape[1]),
+                    _ptr(bw), C.c_int32(K), _ptr(c), _ptr(ws), C.c_int64(ws.numel()), C.c_void_p(s.cuda_stream)),
+                    'metis_het_recost')
+                costs_dev[:, lo:hi] = c
             costs = costs_dev.cpu().numpy()
         t1 = time.perf_counter()
         best, regret = recost_regret(costs_dev)
@@ -671,8 +676,8 @@ class Candidates:
         """Every candidate under the scenario profiles ``problems`` (each flattened under the searched cluster, model
         flags and corrections), with its device groups, strategies and partition held fixed: cost, headroom and status
         per scenario (metis_het_profile_recost), segment by segment, _RECOST_CHUNK records per launch.  The scenarios'
-        tables are uploaded once.  timings: ``recost_s`` up to the arrays on the host, ``regret_s`` the regret kernels
-        and their copy."""
+        tables are uploaded once.  timings: ``recost_s`` up to the arrays on the host, ``regret_s`` the usable mask,
+        the regret kernels and their copy."""
         t0 = time.perf_counter()
         dev = _require_cuda(self.device)
         K, n = len(problems), len(self.records)
@@ -686,23 +691,22 @@ class Candidates:
             costs_dev = torch.empty((K, n), dtype=torch.float64, device=dev)
             head_dev = torch.empty((K, n), dtype=torch.float64, device=dev)
             status_dev = torch.empty((K, n), dtype=torch.uint8, device=dev)
-            for seg in self.segments:
-                if seg.first == seg.end:                      # nothing to replay: a window is not reloaded for it
-                    continue
-                _lib, _p, sp, _ws, _dev, _keep = seg.bind()
-                for lo in range(seg.first, seg.end, _RECOST_CHUNK):
-                    hi = min(seg.end, lo + _RECOST_CHUNK)
-                    rec = self.records[lo:hi]
-                    detail = seg.detail_device(lo - seg.first, hi - seg.first, rec, dev)
-                    c, h, st = het_profile_recost(lib, sp, scen, ws, rec, detail, dev)
-                    costs_dev[:, lo:hi], head_dev[:, lo:hi], status_dev[:, lo:hi] = c, h, st
+            s = torch.cuda.current_stream(dev)
+            for (_lib, _p, sp, _ws, _dev, _keep), lo, hi, rec, detail in self._replay_chunks(dev):
+                c, h = (torch.empty((K, hi - lo), dtype=torch.float64, device=dev) for _ in range(2))
+                st = torch.empty((K, hi - lo), dtype=torch.uint8, device=dev)
+                native.check(lib.metis_het_profile_recost(
+                    C.byref(sp), C.c_void_p(C.addressof(scen)), C.c_int32(K), _ptr(rec), C.c_int64(hi - lo),
+                    _ptr(detail), C.c_int32(detail.shape[1]), _ptr(c), _ptr(h), _ptr(st), _ptr(ws),
+                    C.c_int64(ws.numel()), C.c_void_p(s.cuda_stream)), 'metis_het_profile_recost')
+                costs_dev[:, lo:hi], head_dev[:, lo:hi], status_dev[:, lo:hi] = c, h, st
             costs, headroom, status = costs_dev.cpu().numpy(), head_dev.cpu().numpy(), status_dev.cpu().numpy()
         t1 = time.perf_counter()
-        usable = (status == 0) & (headroom >= 0)
         with torch.cuda.device(dev):
-            # an unusable entry at +inf: fmax would skip a NaN, and a plan that does not fit somewhere would look robust
-            masked = torch.from_numpy(np.where(usable, costs, np.inf)).to(dev)
-            best, regret = recost_regret(masked)
+            # an unusable entry at +inf: fmax would skip a NaN, and a plan that does not fit somewhere would look
+            # robust.  A NaN headroom compares false, so it is unusable.
+            usable = (status_dev == 0) & (head_dev >= 0)
+            best, regret = recost_regret(torch.where(usable, costs_dev, math.inf))
         t2 = time.perf_counter()
         return Recost(self, costs, best, regret, dev, {'recost_s': t1 - t0, 'regret_s': t2 - t1}, headroom, status)
 
@@ -741,27 +745,19 @@ class Candidates:
             regret = torch.full((max(n, 1),), -math.inf, dtype=torch.float64, device=dev)
             total = torch.zeros(max(n, 1), dtype=torch.float64, device=dev)
             s = torch.cuda.current_stream(dev)
-            ptr = lambda t, off=0: C.c_void_p(t.data_ptr() + off)              # noqa: E731
             for first in range(0, samples, chunk):
                 spec.first, spec.count = first, min(chunk, samples - first)
-                native.check(lib.metis_het_profile_noise_draw(C.byref(p), C.byref(spec), ptr(ws), C.c_int64(ws.numel()),
-                                                              C.c_void_p(s.cuda_stream)), 'metis_het_profile_noise_draw')
-                for seg in self.segments:
-                    if seg.first == seg.end:
-                        continue
-                    _lib, _p, sp, _w, _d, _k = seg.bind()
-                    for lo in range(seg.first, seg.end, _RECOST_CHUNK):
-                        hi = min(seg.end, lo + _RECOST_CHUNK)
-                        rec = self.records[lo:hi]
-                        detail = seg.detail_device(lo - seg.first, hi - seg.first, rec, dev)
-                        d_rec = upload(rec, dev)
-                        native.check(lib.metis_het_profile_noise_eval(
-                            C.byref(sp), C.byref(spec), ptr(ws), ptr(d_rec), C.c_int64(hi - lo), ptr(detail),
-                            C.c_int32(detail.shape[1]), ptr(cost, 8 * lo), ptr(usable, lo), C.c_int64(n),
-                            C.c_void_p(s.cuda_stream)), 'metis_het_profile_noise_eval')
+                native.check(lib.metis_het_profile_noise_draw(
+                    C.byref(p), C.byref(spec), _ptr(ws), C.c_int64(ws.numel()), C.c_void_p(s.cuda_stream)),
+                    'metis_het_profile_noise_draw')
+                for (_lib, _p, sp, _w, _d, _k), lo, hi, rec, detail in self._replay_chunks(dev):
+                    native.check(lib.metis_het_profile_noise_eval(
+                        C.byref(sp), C.byref(spec), _ptr(ws), _ptr(rec), C.c_int64(hi - lo), _ptr(detail),
+                        C.c_int32(detail.shape[1]), _ptr(cost, 8 * lo), _ptr(usable, lo), C.c_int64(n),
+                        C.c_void_p(s.cuda_stream)), 'metis_het_profile_noise_eval')
                 native.check(lib.metis_het_profile_noise_reduce(
-                    C.byref(spec), ptr(cost), ptr(usable), C.c_int64(n), ptr(best_pos, 8 * first),
-                    ptr(best_cost, 8 * first), ptr(wins), ptr(near), ptr(count), ptr(regret), ptr(total),
+                    C.byref(spec), _ptr(cost), _ptr(usable), C.c_int64(n), _ptr(best_pos, 8 * first),
+                    _ptr(best_cost, 8 * first), _ptr(wins), _ptr(near), _ptr(count), _ptr(regret), _ptr(total),
                     C.c_void_p(s.cuda_stream)), 'metis_het_profile_noise_reduce')
             out = [t.cpu().numpy() for t in (best_pos, best_cost, wins, near, count, regret, total)]
         best_pos, best_cost, wins, near, count, regret, total = out
@@ -774,10 +770,26 @@ class Candidates:
                             {'noise_s': t1 - t0, 'chunks': -(-samples // chunk), 'chunk': chunk})
 
     def records_device(self) -> torch.Tensor:
-        """The records (estimate_costs order) on the device, uploaded on first use: what the group passes read."""
+        """The records (estimate_costs order) on the device, uploaded on first use: what the replays and the group
+        passes read."""
         if getattr(self, '_records_dev', None) is None:
             self._records_dev = upload(self.records, _require_cuda(self.device))
         return self._records_dev
+
+    def _replay_chunks(self, dev, with_detail: bool = True):
+        """Every non-empty segment's records, _RECOST_CHUNK at a time: (the segment's bound structs (``bind()``), lo,
+        hi, the device bytes of the records [lo, hi) (records_device), their device detail rows, or None without
+        ``with_detail``).  An empty segment is skipped: a window is not reloaded for it."""
+        recs, width = self.records_device(), self.records.itemsize
+        for seg in self.segments:
+            if seg.first == seg.end:
+                continue
+            bound = seg.bind()
+            for lo in range(seg.first, seg.end, _RECOST_CHUNK):
+                hi = min(seg.end, lo + _RECOST_CHUNK)
+                detail = seg.detail_device(lo - seg.first, hi - seg.first, self.records[lo:hi], dev) \
+                    if with_detail else None
+                yield bound, lo, hi, recs[width * lo:width * hi], detail
 
     def query(self, flt: native.MetisPlanFilter, reads_tp: bool, headroom: Optional[torch.Tensor] = None,
               min_headroom: float = 0.0, groups: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
@@ -788,26 +800,17 @@ class Candidates:
         dev = _require_cuda(self.device)
         n = len(self.records)
         with torch.cuda.device(dev):
-            recs = self.records_device()
             mask = torch.zeros(max(n, 1), dtype=torch.uint8, device=dev)
             group = torch.empty(max(n, 1), dtype=torch.int32, device=dev) if groups else None
             s = torch.cuda.current_stream(dev)
-            for seg in self.segments:
-                if seg.first == seg.end:                      # nothing to mark: a window is not reloaded for it
-                    continue
-                lib, p, sp, _ws, _dev, _keep = seg.bind()
-                for lo in range(seg.first, seg.end, _RECOST_CHUNK):
-                    hi = min(seg.end, lo + _RECOST_CHUNK)
-                    detail = seg.detail_device(lo - seg.first, hi - seg.first, self.records[lo:hi], dev) \
-                        if reads_tp else None
-                    rc = lib.metis_query_mark(
-                        C.byref(p), C.byref(sp), C.byref(flt), C.c_void_p(recs.data_ptr() + 16 * lo), C.c_int64(hi - lo),
-                        C.c_void_p(detail.data_ptr() if detail is not None else 0),
-                        C.c_int32(detail.shape[1] if detail is not None else 0),
-                        C.c_void_p(headroom.data_ptr() + 8 * lo if headroom is not None else 0), C.c_double(min_headroom),
-                        C.c_void_p(mask.data_ptr() + lo), C.c_void_p(group.data_ptr() + 4 * lo if groups else 0),
-                        C.c_void_p(s.cuda_stream))
-                    native.check(rc, 'metis_query_mark')
+            for (lib, p, sp, _ws, _dev, _keep), lo, hi, rec, detail in self._replay_chunks(dev, reads_tp):
+                rc = lib.metis_query_mark(
+                    C.byref(p), C.byref(sp), C.byref(flt), _ptr(rec), C.c_int64(hi - lo),
+                    C.c_void_p(detail.data_ptr() if detail is not None else 0),
+                    C.c_int32(detail.shape[1] if detail is not None else 0),
+                    C.c_void_p(headroom.data_ptr() + 8 * lo if headroom is not None else 0), C.c_double(min_headroom),
+                    _ptr(mask, lo), C.c_void_p(group.data_ptr() + 4 * lo if groups else 0), C.c_void_p(s.cuda_stream))
+                native.check(rc, 'metis_query_mark')
         return mask, group
 
 
@@ -1257,52 +1260,7 @@ def het_breakdown(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.
                 stages[dest[lo:hi]] = d_st.cpu().numpy().reshape(hi - lo, native.BD_FIELDS, width)
 
 
-_RECOST_CHUNK = 1 << 20                   # records per metis_het_recost launch: bounds a window's replayed detail rows
-
-
-def het_recost(lib, p_struct, s_struct, workspace: torch.Tensor, records: np.ndarray, detail: torch.Tensor,
-               bandwidths: torch.Tensor, device) -> torch.Tensor:
-    """metis_het_recost of ``records`` (host MetisRecord rows) with their detail rows (device uint8 [n, stride]) under
-    the scenarios ``bandwidths`` (device float64 [K, 2, num_types]) on the bound problem / space; returns the device
-    costs [K, n].  Asynchronous on the current stream."""
-    n, K = len(records), int(bandwidths.shape[0])
-    with torch.cuda.device(device):
-        costs = torch.empty((K, n), dtype=torch.float64, device=device)
-        if n == 0:
-            return costs
-        d_rec = upload(records, device)
-        s = torch.cuda.current_stream(device)
-        rc = lib.metis_het_recost(C.byref(p_struct), C.byref(s_struct), C.c_void_p(d_rec.data_ptr()), C.c_int64(n),
-                                  C.c_void_p(detail.data_ptr()), C.c_int32(detail.shape[1]),
-                                  C.c_void_p(bandwidths.data_ptr()), C.c_int32(K), C.c_void_p(costs.data_ptr()),
-                                  C.c_void_p(workspace.data_ptr()), C.c_int64(workspace.numel()),
-                                  C.c_void_p(s.cuda_stream))
-        native.check(rc, 'metis_het_recost')
-    return costs
-
-
-def het_profile_recost(lib, s_struct, scenarios, workspace: torch.Tensor, records: np.ndarray, detail: torch.Tensor,
-                       device) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-    """metis_het_profile_recost of ``records`` (host MetisRecord rows) with their detail rows (device uint8 [n, stride])
-    on the bound space under the scenario problems ``scenarios`` (a ctypes array of MetisProblem bound on the device);
-    returns the device costs, headroom and status [K, n].  Asynchronous on the current stream."""
-    n, K = len(records), len(scenarios)
-    with torch.cuda.device(device):
-        costs = torch.empty((K, n), dtype=torch.float64, device=device)
-        headroom = torch.empty((K, n), dtype=torch.float64, device=device)
-        status = torch.empty((K, n), dtype=torch.uint8, device=device)
-        if n == 0:
-            return costs, headroom, status
-        d_rec = upload(records, device)
-        s = torch.cuda.current_stream(device)
-        rc = lib.metis_het_profile_recost(C.byref(s_struct), C.c_void_p(C.addressof(scenarios)), C.c_int32(K),
-                                          C.c_void_p(d_rec.data_ptr()), C.c_int64(n), C.c_void_p(detail.data_ptr()),
-                                          C.c_int32(detail.shape[1]), C.c_void_p(costs.data_ptr()),
-                                          C.c_void_p(headroom.data_ptr()), C.c_void_p(status.data_ptr()),
-                                          C.c_void_p(workspace.data_ptr()), C.c_int64(workspace.numel()),
-                                          C.c_void_p(s.cuda_stream))
-        native.check(rc, 'metis_het_profile_recost')
-    return costs, headroom, status
+_RECOST_CHUNK = 1 << 20                   # records per replay launch: bounds a window's replayed detail rows
 
 
 def recost_regret(costs: torch.Tensor) -> Tuple[np.ndarray, np.ndarray]:
