@@ -409,6 +409,33 @@ int metis_het_profile_noise_reduce(const MetisNoiseSpec *spec, const double *cos
                                    int32_t *usable_count, double *regret, double *sum, void *stream);
 
 /*
+ * Search what-if: a fresh search under each seeded sample of the profile (search.noisy_profile), the balancer's layer
+ * weights included.  The draw is metis_het_profile_noise_draw's, and it also writes each sample's norm_lc
+ * (load_balancer.py:22-27, quirk Q3): the tp1_bs1 layer-computes of the profile's FIRST-LISTED entry, which need not be
+ * a device type of the cluster, each multiplied by its factor (field 1, tp 1, bs 1, that entry's device type), then
+ * each divided by their CPython sum.  Under sigma 0 for that entry's layer-computes it is the base's norm_lc.  The
+ * workspace's descriptors at its start serve metis_het_profile_noise_eval as after metis_het_profile_noise_draw, and
+ * metis_het_search_noise_problem gives sample s's MetisProblem (device pointers into the workspace) for
+ * metis_het_search / metis_het_detail.  The workspace must not change while those run.
+ */
+typedef struct MetisNormSource {
+    const double *row;            /* [device] len doubles: the first-listed entry's tp1_bs1 'layer-computes'         */
+    int32_t len;                  /* == base->norm_len                                                            */
+    int32_t type_code;            /* 1-based utils.DeviceType position of that entry's device type (1 .. 6)       */
+    double sigma;                 /* its layer-computes sigma, finite, in [0, 1)                                  */
+} MetisNormSource;
+
+/* workspace bytes of one chunk of `count` samples of `base`, or METIS_E_ARG */
+int64_t metis_het_search_noise_workspace_bytes(const MetisProblem *base, int32_t count);
+/* norm_zero [device] spec->count bytes: 1 where the sample's noisy norm total is 0 (the reference raises
+ * ZeroDivisionError; that sample's norm_lc is then the base's), else 0.  spec->near_factor is checked, not read. */
+int metis_het_search_noise_draw(const MetisProblem *base, const MetisNoiseSpec *spec, const MetisNormSource *norm,
+                                void *workspace, int64_t workspace_bytes, uint8_t *norm_zero, void *stream);
+/* host only: sample s (0 <= s < spec->count) of the chunk drawn into workspace with the same base and spec */
+int metis_het_search_noise_problem(const MetisProblem *base, const MetisNoiseSpec *spec, int32_t s,
+                                   const void *workspace, MetisProblem *sample);
+
+/*
  * metis_homo_cost with the cost terms and the per-stage memory sums (HomoCostEstimator.get_cost returns them as
  * stage_memory, model/cost_estimator.py:121-138).
  *   terms        [device] n x 6 doubles: execution, fb_sync, parameter update, dp, pp, batch generate

@@ -189,6 +189,7 @@ class HetSearchResult(Sequence):
         # (cluster, model_config, gbs, max_tp, max_bs, node_sequences, corrected) the search flattened its profile
         # under (cost_het_cluster sets it): a profile what-if flattens its scenarios the same way
         self._flat_inputs = None
+        self._norm_source = None              # norm_source() of the searched profile (cost_het_cluster sets it)
 
     def __len__(self) -> int:
         return len(self.candidates)
@@ -481,6 +482,12 @@ class HetSearchResult(Sequence):
         searched profile.  This is not a search under each sample.  ValueError for samples outside 1 .. 65535, a
         sigma, seed or within out of range, or an unknown field or device type.  With torch.distributed every rank
         computes locally: no collective is issued."""
+        table, codes, seed, _sig = self._noise_args(samples, sigma, seed, within)
+        return self.candidates.profile_noise(table, codes, seed, samples, float(within))
+
+    def _noise_args(self, samples: int, sigma, seed: int, within: float):
+        """The checked arguments of a noise what-if: (sigma table [3, METIS_MAX_TYPES] and device type codes per device
+        type of the searched problem, the seed, noise_sigmas(sigma))."""
         from . import search
         if not isinstance(samples, int) or isinstance(samples, bool) or not 1 <= samples <= search.MAX_NOISE_SAMPLES:
             raise ValueError(f'samples must be an int in [1, {search.MAX_NOISE_SAMPLES}], not {samples!r}')
@@ -494,17 +501,83 @@ class HetSearchResult(Sequence):
         for f, field in enumerate(search.NOISE_FIELDS):
             for t, name in enumerate(problem.type_names):
                 table[f, t] = search._sigma_of(sig, field, name)
-        return self.candidates.profile_noise(table, codes, seed, samples, float(within))
+        return table, codes, seed, sig
+
+    def search_noise(self, samples: int, sigma, seed: int = 0, within: float = 0.01) -> 'search.ScenarioSearch':
+        """Search what-if under profile noise: a fresh search under each of ``samples`` seeded samples of the searched
+        profile, ``search.noisy_profile(profile, sigma, seed, j)`` as profile_noise draws them, with the balancer's
+        layer weights (norm_lc) of the sample too, next to the searched best held fixed.  Sample j's search is
+        bit for bit what cost_het_cluster returns under that sample's dict with the searched args, cluster, node
+        sequences and corrections and a HeteroCostEstimator and LayerLoadBalancer built from the dict.  Returns a
+        search.ScenarioSearch: each sample's status, candidate count, winner and best cost, the searched best's cost
+        and fit under it, the loss of keeping the searched best and whether it stays ``within`` of the winner.  Under
+        all-zero sigma every sample's search is this result's.  The same ValueErrors as profile_noise;
+        NotImplementedError for a result searched in more than one window.  With torch.distributed every rank
+        computes locally: no collective is issued."""
+        from . import search
+        table, codes, seed, sig = self._noise_args(samples, sigma, seed, within)
+        if self._norm_source is None:
+            raise ValueError('this result does not know the profile entry its layer weights come from: no search_noise')
+        name, row = self._norm_source
+        problem = self.candidates.problem
+        s, code = 0.0, 1
+        if name.startswith('DeviceType.'):
+            tname = name[len('DeviceType.'):]
+            if any(search._sigma_of(sig, f, tname) for f in search.NOISE_FIELDS):
+                code = search.device_type_code(tname)            # noisy_profile refuses an unknown type the same way
+            s = search._sigma_of(sig, 'layer-computes', tname)
+        if s and len(row) != problem.scalars['norm_len']:
+            raise ValueError(f"the searched layer weights have {problem.scalars['norm_len']} entries, the profile's "
+                             f'first entry {name} has {len(row)}: not the profile the balancer was built from')
+        spec = search.noise_spec(table, codes, seed, within)
+        scen = search.NoiseScenarios(spec, samples, row if s else None, code, float(s))
+        return self.candidates.search_scenarios(scen, self._best_position(), float(within))
+
+    def search_profiles(self, profiles: Sequence[Dict], within: float = 0.01) -> 'search.ScenarioSearch':
+        """Search what-if under given profiles: a fresh search under each profile of ``profiles``, flattened under
+        the searched args, cluster, node sequences and corrections with its own layer weights (norm_lc, from its
+        first-listed entry), next to the searched best held fixed, evaluated as recost_profiles evaluates it.  Returns
+        a search.ScenarioSearch as search_noise does; a profile whose layer-weight total is 0 has the status
+        METIS_FATAL_ZERODIV.  The same ValueErrors as recost_profiles; NotImplementedError for a result searched in
+        more than one window.  With torch.distributed every rank computes locally: no collective is issued."""
+        from . import search
+        if self._flat_inputs is None:
+            raise ValueError('this result does not know the inputs it was searched on: no search_profiles')
+        profiles = list(profiles)
+        if not profiles:
+            raise ValueError('search_profiles needs at least one profile')
+        if not search._real(within) or not math.isfinite(within) or within < 0:
+            raise ValueError(f'within must be a finite number >= 0, not {within!r}')
+        cluster, model_config, gbs, max_tp, max_bs, seqs, corrected = self._flat_inputs
+        problem = self.candidates.problem
+        for j, prof in enumerate(profiles):
+            check_profile(prof, problem.type_names, j)
+        scen, zerodiv = [], []
+        for prof in profiles:
+            try:
+                norm, zero = flatten.norm_layer_duration(prof), False
+            except ZeroDivisionError:                     # LayerLoadBalancer(prof) raises: nothing is searched
+                norm, zero = problem.arrays['norm_lc'], True
+            zerodiv.append(zero)
+            scen.append(flatten.build_problem(prof, cluster, model_config, gbs, max_tp, max_bs, seqs, norm,
+                                              corrected=corrected))
+        return self.candidates.search_scenarios(search.ProfileScenarios(scen, zerodiv), self._best_position(),
+                                                float(within))
+
+    def _best_position(self) -> Optional[int]:
+        """The position of best() in estimate_costs order, or None for an empty result."""
+        if self.rank_order is None and self._best_key is not None and len(self):
+            at = self.candidates.index_of(*self._best_key)    # records sorted by (ordinal, step): no temporaries
+            if at is not None:
+                return at
+        order = self._rank()
+        return int(order[0]) if len(order) else None
 
     def best(self) -> Optional[Tuple]:
         """argmin (cost, position): the first entry of the ranked list.  The search kernels reduce it on the device
         (het_finalize_kernel: lowest cost, then lowest ordinal, then lowest step), so no sort is needed for it."""
-        if self.rank_order is None and self._best_key is not None and len(self):
-            at = self.candidates.index_of(*self._best_key)    # records sorted by (ordinal, step): no temporaries
-            if at is not None:
-                return self.candidates.tuples([at])[0]
-        top = self.ranked(1)
-        return top[0] if top else None
+        at = self._best_position()
+        return self.candidates.tuples([at])[0] if at is not None else None
 
 
 def cluster_signature(gpu_cluster, type_names: Sequence[str]) -> Tuple[list, list]:
@@ -721,7 +794,18 @@ def cost_het_cluster(args: argparse.Namespace, gpu_cluster, profile_data: Dict, 
     result._searched = cluster_signature(gpu_cluster, problem.type_names)
     result._flat_inputs = (gpu_cluster, model_config, args.gbs, args.max_profiled_tp_degree,
                            args.max_profiled_batch_size, [tuple(s) for s in node_sequences], tuple(corrected))
+    result._norm_source = norm_source(profile_data)
     return result
+
+
+def norm_source(profile_data) -> Optional[Tuple[str, np.ndarray]]:
+    """What flatten.norm_layer_duration reads (model/load_balancer.py:22-27, quirk Q3): the profile's first-listed
+    entry's name and a copy of its tp1_bs1 layer-computes, or None when it has none."""
+    try:
+        first = next(iter(profile_data))
+        return first, np.array(profile_data[first]['tp1_bs1']['time']['layer-computes'], dtype=np.float64)
+    except (StopIteration, KeyError, TypeError, ValueError):
+        return None
 
 
 def _one_search(problem, space, seqs, dev, rank: int, world: int, headroom: bool, misses: bool):

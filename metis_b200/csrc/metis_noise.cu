@@ -14,6 +14,10 @@
 //                            holds it (group_min_kernel / group_first_kernel's two passes, with a warp's minimum taken
 //                            before its one atomicMin)
 //   noise_accumulate_kernel  one thread per candidate, the chunk's samples in order: noise_accumulate (metis_noise.cuh)
+//
+// Search what-if (metis_het_search_noise_*): the same draw, each sample's norm_lc included, for a fresh search per sample.
+//   noise_norm_kernel        one thread per sample: noisy_norm (metis_noise.cuh) of the profile's first-listed tp1_bs1
+//                            row, the base's norm_lc when its sigma is 0 or when the noisy total is 0 (then flagged)
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -31,18 +35,19 @@ namespace metis {
 constexpr int kReduceThreads = 256;
 constexpr int kMaxSamples = 65535;
 
-// Where a chunk's pieces sit in the workspace (from its 256-aligned start)
+// Where a chunk's pieces sit in the workspace (from its 256-aligned start).  A sample's arrays are its layer_compute,
+// layer_memory, exec_full and fb_sync, then, with `norm_len` > 0 (the search what-if), its norm_lc.
 struct NoiseLayout {
     int64_t desc, meta, arrays, array_stride, replay, replay_stride, total;
 };
 
-static NoiseLayout noise_layout(const MetisProblem &b, int count, int64_t replay_bytes) {
+static NoiseLayout noise_layout(const MetisProblem &b, int count, int64_t replay_bytes, int norm_len = 0) {
     NoiseLayout l;
     const int64_t K = b.num_keys, row = (int64_t)b.num_keys * b.lpad;
     l.desc = 0;
     l.meta = align256((int64_t)count * (int64_t)sizeof(ScenarioTables));
     l.arrays = l.meta + align256(K * 4);
-    l.array_stride = align256((2 * row + 2 * K) * (int64_t)sizeof(double));
+    l.array_stride = align256((2 * row + 2 * K + norm_len) * (int64_t)sizeof(double));
     l.replay = l.arrays + (int64_t)count * l.array_stride;
     l.replay_stride = align256(replay_bytes);
     l.total = l.replay + (int64_t)count * l.replay_stride + 256;
@@ -85,6 +90,20 @@ noise_keys_kernel(const __grid_constant__ MetisProblem b, const __grid_constant_
     ef[k] = spec.sigma[0][m & 0xff] == 0.0 ? b.exec_full[k] : noisy_exec_full(lc + (long long)k * b.lpad, b.lpad);
     fb[k] = noisy_value(b.fb_sync[k], spec.sigma[2], spec.type_code, spec.seed, (uint32_t)(spec.first + s), m,
                         kNoiseFbSync, 0);
+}
+
+__global__ void __launch_bounds__(kReduceThreads)
+noise_norm_kernel(const __grid_constant__ MetisProblem b, const __grid_constant__ MetisNoiseSpec spec,
+                  const __grid_constant__ MetisNormSource src, uint8_t *arrays, long long array_stride,
+                  long long norm_at, uint8_t *zero) {
+    const int s = blockIdx.x * kReduceThreads + threadIdx.x;
+    if (s >= spec.count) return;
+    double *out = reinterpret_cast<double *>(arrays + s * array_stride + norm_at);
+    const bool drawn = src.sigma != 0.0 &&
+                       noisy_norm(src.row, src.len, src.sigma, spec.seed, (uint32_t)(spec.first + s), src.type_code, out);
+    if (!drawn)
+        for (int i = 0; i < b.norm_len; ++i) out[i] = b.norm_lc[i];
+    zero[s] = src.sigma != 0.0 && !drawn;
 }
 
 __device__ __forceinline__ unsigned long long warp_min(unsigned long long v) {
@@ -180,6 +199,56 @@ static const char *check_spec(const MetisNoiseSpec *spec, int num_types) {
     return nullptr;
 }
 
+// Sample s of a chunk drawn into `ws` (layout `lay`): `base` with its drawn tables, norm_lc too when `own_norm`
+static MetisProblem sample_problem(const MetisProblem &base, const NoiseLayout &lay, const uint8_t *ws, int s,
+                                   bool own_norm) {
+    MetisProblem p = base;
+    const int64_t row = (int64_t)base.num_keys * base.lpad;
+    const double *lc = reinterpret_cast<const double *>(ws + lay.arrays + (int64_t)s * lay.array_stride);
+    p.layer_compute = lc;
+    p.layer_memory = lc + row;
+    p.exec_full = lc + 2 * row;
+    p.fb_sync = lc + 2 * row + base.num_keys;
+    if (own_norm) p.norm_lc = lc + 2 * row + 2 * base.num_keys;
+    return p;
+}
+
+// The chunk's layer_compute, layer_memory, exec_full and fb_sync from the base's, then every sample's tables packed
+// and their descriptors written (stage_scenarios).  A search what-if has launched noise_norm_kernel before.
+static int draw_chunk(const MetisProblem &base, const MetisNoiseSpec &spec, const NoiseLayout &lay, uint8_t *ws,
+                      bool own_norm, cudaStream_t stream) {
+    uint32_t *meta = reinterpret_cast<uint32_t *>(ws + lay.meta);
+    uint8_t *arrays = ws + lay.arrays;
+    const int count = spec.count;
+    key_meta_kernel<<<blocks_of((long long)base.num_types * base.num_tp * base.num_bs, kReduceThreads),
+                      kReduceThreads, 0, stream>>>(base, meta);
+    const long long row = (long long)base.num_keys * base.lpad;
+    noise_rows_kernel<<<dim3(blocks_of(row, kReduceThreads), count), kReduceThreads, 0, stream>>>(
+        base, spec, meta, arrays, lay.array_stride);
+    noise_keys_kernel<<<dim3(blocks_of(base.num_keys, kReduceThreads), count), kReduceThreads, 0, stream>>>(
+        base, spec, meta, arrays, lay.array_stride);
+    std::vector<MetisProblem> samples((size_t)count);
+    for (int s = 0; s < count; ++s) samples[(size_t)s] = sample_problem(base, lay, ws, s, own_norm);
+    return stage_scenarios(samples.data(), count, reinterpret_cast<ScenarioTables *>(ws + lay.desc), ws + lay.replay,
+                           stream);
+}
+
+// The layout of a search what-if chunk, or why it cannot be drawn
+static const char *search_noise_layout(const MetisProblem *base, const MetisNoiseSpec *spec, NoiseLayout &lay,
+                                       int &rc) {
+    rc = METIS_E_ARG;
+    if (base->num_types < 1 || base->num_types > METIS_MAX_TYPES) return "num_types out of range";
+    if (const char *why = check_spec(spec, base->num_types)) return why;
+    const int64_t replay = replay_tables_bytes(base);
+    if (replay < 0) {
+        rc = (int)replay;
+        return "bad base problem";
+    }
+    lay = noise_layout(*base, spec->count, replay, base->norm_len);
+    rc = METIS_OK;
+    return nullptr;
+}
+
 }  // namespace metis
 
 using namespace metis;
@@ -203,31 +272,52 @@ int metis_het_profile_noise_draw(const MetisProblem *base, const MetisNoiseSpec 
     if (replay < 0) return (int)replay;
     const NoiseLayout lay = noise_layout(*base, spec->count, replay);
     if (workspace_bytes < lay.total) return METIS_E_CAPACITY;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    uint8_t *ws = align_workspace(workspace);
-    uint32_t *meta = reinterpret_cast<uint32_t *>(ws + lay.meta);
-    uint8_t *arrays = ws + lay.arrays;
-    const int count = spec->count;
-    key_meta_kernel<<<blocks_of((long long)base->num_types * base->num_tp * base->num_bs, kReduceThreads),
-                      kReduceThreads, 0, stream>>>(*base, meta);
-    const long long row = (long long)base->num_keys * base->lpad;
-    noise_rows_kernel<<<dim3(blocks_of(row, kReduceThreads), count), kReduceThreads, 0, stream>>>(
-        *base, *spec, meta, arrays, lay.array_stride);
-    noise_keys_kernel<<<dim3(blocks_of(base->num_keys, kReduceThreads), count), kReduceThreads, 0, stream>>>(
-        *base, *spec, meta, arrays, lay.array_stride);
-    std::vector<MetisProblem> samples((size_t)count, *base);
-    for (int s = 0; s < count; ++s) {
-        const double *lc = reinterpret_cast<const double *>(arrays + (int64_t)s * lay.array_stride);
-        samples[(size_t)s].layer_compute = lc;
-        samples[(size_t)s].layer_memory = lc + row;
-        samples[(size_t)s].exec_full = lc + 2 * row;
-        samples[(size_t)s].fb_sync = lc + 2 * row + base->num_keys;
-    }
-    const int rc = stage_scenarios(samples.data(), count, reinterpret_cast<ScenarioTables *>(ws + lay.desc),
-                                   ws + lay.replay, stream);
+    const int rc = draw_chunk(*base, *spec, lay, align_workspace(workspace), false, static_cast<cudaStream_t>(stream_));
     if (rc) return rc;
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? METIS_OK : fail_cuda(e, "metis_het_profile_noise_draw");
+}
+
+int64_t metis_het_search_noise_workspace_bytes(const MetisProblem *base, int32_t count) {
+    if (!base || count < 1 || count > kMaxSamples) return METIS_E_ARG;
+    const int64_t b = replay_tables_bytes(base);
+    if (b < 0) return b;
+    return noise_layout(*base, count, b, base->norm_len).total;
+}
+
+int metis_het_search_noise_draw(const MetisProblem *base, const MetisNoiseSpec *spec, const MetisNormSource *norm,
+                                void *workspace, int64_t workspace_bytes, uint8_t *norm_zero, void *stream_) {
+    if (!base || !spec || !norm || !norm->row || !workspace || !norm_zero)
+        return fail_arg("metis_het_search_noise_draw: NULL argument");
+    NoiseLayout lay;
+    int rc;
+    if (const char *why = search_noise_layout(base, spec, lay, rc)) return rc == METIS_E_ARG ? fail_arg(why) : rc;
+    if (norm->len != base->norm_len) return fail_arg("metis_het_search_noise_draw: norm->len != base->norm_len");
+    if (norm->type_code < 1 || norm->type_code > 6)
+        return fail_arg("metis_het_search_noise_draw: norm->type_code out of range (1 .. 6)");
+    if (!(norm->sigma >= 0.0 && norm->sigma < 1.0))
+        return fail_arg("metis_het_search_noise_draw: norm->sigma must be finite and in [0, 1)");
+    if (workspace_bytes < lay.total) return METIS_E_CAPACITY;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    uint8_t *ws = align_workspace(workspace);
+    const long long norm_at = (2LL * base->num_keys * base->lpad + 2LL * base->num_keys) * (long long)sizeof(double);
+    noise_norm_kernel<<<blocks_of(spec->count, kReduceThreads), kReduceThreads, 0, stream>>>(
+        *base, *spec, *norm, ws + lay.arrays, lay.array_stride, norm_at, norm_zero);
+    rc = draw_chunk(*base, *spec, lay, ws, true, stream);
+    if (rc) return rc;
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? METIS_OK : fail_cuda(e, "metis_het_search_noise_draw");
+}
+
+int metis_het_search_noise_problem(const MetisProblem *base, const MetisNoiseSpec *spec, int32_t s,
+                                   const void *workspace, MetisProblem *sample) {
+    if (!base || !spec || !workspace || !sample) return fail_arg("metis_het_search_noise_problem: NULL argument");
+    NoiseLayout lay;
+    int rc;
+    if (const char *why = search_noise_layout(base, spec, lay, rc)) return rc == METIS_E_ARG ? fail_arg(why) : rc;
+    if (s < 0 || s >= spec->count) return fail_arg("metis_het_search_noise_problem: sample out of range (0 .. count-1)");
+    *sample = sample_problem(*base, lay, align_workspace(const_cast<void *>(workspace)), s, true);
+    return METIS_OK;
 }
 
 int metis_het_profile_noise_eval(const MetisPlanSpace *space, const MetisNoiseSpec *spec, const void *workspace,

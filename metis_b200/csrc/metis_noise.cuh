@@ -22,11 +22,13 @@ enum NoiseField { kNoiseCompute = 1, kNoiseMemory = 2, kNoiseFbSync = 3 };
 MB_HD double noise_mul(double a, double b) { return __dmul_rn(a, b); }
 MB_HD double noise_add(double a, double b) { return __dadd_rn(a, b); }
 MB_HD double noise_sub(double a, double b) { return __dsub_rn(a, b); }
+MB_HD double noise_div(double a, double b) { return __ddiv_rn(a, b); }
 MB_HD uint32_t mulhi32(uint32_t a, uint32_t b) { return __umulhi(a, b); }
 #else
 MB_HD double noise_mul(double a, double b) { return a * b; }
 MB_HD double noise_add(double a, double b) { return a + b; }
 MB_HD double noise_sub(double a, double b) { return a - b; }
+MB_HD double noise_div(double a, double b) { return a / b; }
 MB_HD uint32_t mulhi32(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) >> 32); }
 #endif
 
@@ -78,6 +80,23 @@ MB_HD double noisy_exec_full(const double *row, int lpad) {
     PySum s;
     for (int l = 0; l < lpad; ++l) s.add(row[l]);
     return s.result();
+}
+
+// Sample j's norm_lc, the balancer's layer weights (load_balancer.py:22-27, quirk Q3) under noisy_profile: `row` the
+// n layer-computes of the profile's first-listed entry's tp1_bs1 (device type `type`, 1-based utils.DeviceType
+// position, layer-computes sigma `s` > 0), each multiplied by its factor (tp 1, bs 1, field 1), then each product divided
+// by their CPython sum.  Returns false, with `out` holding the products, when that sum is 0: the reference's
+// ZeroDivisionError.
+MB_HD bool noisy_norm(const double *row, int n, double s, uint64_t seed, uint32_t j, int type, double *out) {
+    PySum total;
+    for (int i = 0; i < n; ++i) {
+        out[i] = noise_mul(row[i], noise_factor(s, seed, j, (uint32_t)i, 1, kNoiseCompute, type, 0));
+        total.add(out[i]);
+    }
+    const double t = total.result();
+    if (t == 0.0) return false;
+    for (int i = 0; i < n; ++i) out[i] = noise_div(out[i], t);
+    return true;
 }
 
 // The running per-candidate statistics of one sample: `u` whether the candidate is usable, `c` its cost, `is_best`

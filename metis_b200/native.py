@@ -19,6 +19,7 @@ METIS_MAX_PERMUTE_GROUPS = 32
 DETAIL_STRIDE = 3 * METIS_MAX_STAGES + 1
 
 FATAL_NAMES = {1: 'KEY_EXEC', 2: 'KEY_MEMORY', 3: 'INDEX', 4: 'HANG', 5: 'SCRATCH', 6: 'ZERODIV'}
+FATAL_ZERODIV = 6                              # METIS_FATAL_ZERODIV
 
 
 class MetisProblem(C.Structure):
@@ -78,6 +79,10 @@ class MetisNoiseSpec(C.Structure):
                 ('count', C.c_int32), ('type_code', C.c_uint8 * METIS_MAX_TYPES), ('near_factor', C.c_double)]
 
 
+class MetisNormSource(C.Structure):
+    _fields_ = [('row', C.c_void_p), ('len', C.c_int32), ('type_code', C.c_int32), ('sigma', C.c_double)]
+
+
 class MetisPlanFilter(C.Structure):
     _fields_ = [('min_stages', C.c_int32), ('max_stages', C.c_int32), ('max_repartition', C.c_int32),
                 ('max_tp_code', C.c_int32), ('uniform_tp', C.c_int32), ('flags', C.c_int32),
@@ -115,7 +120,8 @@ SYMBOLS = ['metis_last_error', 'metis_abi_version', 'metis_set_profile_events', 
            'metis_recost_regret', 'metis_query_mark', 'metis_query_groups', 'metis_mask_select',
            'metis_het_profile_recost_workspace_bytes', 'metis_het_profile_recost',
            'metis_het_profile_noise_workspace_bytes', 'metis_het_profile_noise_draw', 'metis_het_profile_noise_eval',
-           'metis_het_profile_noise_reduce']
+           'metis_het_profile_noise_reduce', 'metis_het_search_noise_workspace_bytes', 'metis_het_search_noise_draw',
+           'metis_het_search_noise_problem']
 SORT_POSITION, SORT_RANKED, SORT_BY_COST_STABLE = 0, 1, 2
 
 _lib = None
@@ -197,6 +203,15 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
     lib.metis_het_profile_noise_reduce.restype = C.c_int
     lib.metis_het_profile_noise_reduce.argtypes = [C.POINTER(MetisNoiseSpec)] + [C.c_void_p] * 2 + [C.c_int64] + \
         [C.c_void_p] * 8
+    lib.metis_het_search_noise_workspace_bytes.restype = C.c_int64
+    lib.metis_het_search_noise_workspace_bytes.argtypes = [C.POINTER(MetisProblem), C.c_int32]
+    lib.metis_het_search_noise_draw.restype = C.c_int
+    lib.metis_het_search_noise_draw.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisNoiseSpec),
+                                                C.POINTER(MetisNormSource), C.c_void_p, C.c_int64, C.c_void_p,
+                                                C.c_void_p]
+    lib.metis_het_search_noise_problem.restype = C.c_int
+    lib.metis_het_search_noise_problem.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisNoiseSpec), C.c_int32,
+                                                   C.c_void_p, C.POINTER(MetisProblem)]
     lib.metis_query_mark.restype = C.c_int
     lib.metis_query_mark.argtypes = [C.POINTER(MetisProblem), C.POINTER(MetisPlanSpace), C.POINTER(MetisPlanFilter),
                                      C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_void_p,

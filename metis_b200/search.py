@@ -721,14 +721,7 @@ class Candidates:
         t0 = time.perf_counter()
         dev = _require_cuda(self.device)
         n = len(self.records)
-        spec = native.MetisNoiseSpec()
-        for f in range(3):
-            for t in range(native.METIS_MAX_TYPES):
-                spec.sigma[f][t] = float(sigma[f][t])
-        for t, code in enumerate(type_code):
-            spec.type_code[t] = int(code)
-        spec.seed = int(seed)
-        spec.near_factor = 1.0 + float(within)
+        spec = noise_spec(sigma, type_code, seed, within)
         with torch.cuda.device(dev):
             lib, p, _sp, _ws, _keep = bind_problem(self.problem, dev, workspace=False)
             one = int(lib.metis_het_profile_noise_workspace_bytes(C.byref(p), 1))
@@ -768,6 +761,80 @@ class Candidates:
         return ProfileNoise(self, best_pos, best_cost, wins.astype(np.int64), near.astype(np.int64),
                             count.astype(np.int64), regret, mean,
                             {'noise_s': t1 - t0, 'chunks': -(-samples // chunk), 'chunk': chunk})
+
+    def search_scenarios(self, scenarios, kept: Optional[int], within: float) -> 'ScenarioSearch':
+        """A fresh search of this result's plan space under each of ``scenarios`` (NoiseScenarios or
+        ProfileScenarios), and the candidate at position ``kept`` (the searched best; None when there is none) under
+        each with its device groups, strategies and partition held fixed.  Per chunk of scenarios, on one stream: the
+        scenarios' tables are staged, each is searched best-only (metis_het_search, no records) into its own pinned
+        summary slot, the kept candidate is evaluated under all of them (het_profile_kernel), then one synchronise;
+        each scenario's best is replayed under its own tables (metis_het_detail) before the next chunk is staged.
+        Chunks are sized by _SCENARIO_BUDGET_BYTES; the results do not depend on it.  Owns its buffers: the cached
+        search engine of api.cost_het_cluster is not touched.  timings: ``search_s`` the whole call, ``chunks``."""
+        t0 = time.perf_counter()
+        seg = one_search_segment(self)
+        dev = _require_cuda(self.device)
+        K = scenarios.count
+        size = C.sizeof(native.MetisSearchSummary)
+        with torch.cuda.device(dev):
+            lib, p, sp, _ws, _dev, _keep = seg.bind()
+            stride = 3 * int(sp.max_stage) + 1
+            shard = native.MetisShard(0, 1, 128, 0)
+            slots = -(-int(sp.num_plans) // 128) * 128
+            chunk = scenarios.reserve(lib, p, dev)
+            sws = torch.empty(scenarios.search_bytes(lib, p, slots, int(sp.max_stage)), dtype=torch.uint8, device=dev)
+            summaries = torch.zeros(K * size, dtype=torch.uint8).pin_memory()
+            picks_host = torch.zeros(K * 16, dtype=torch.uint8).pin_memory()
+            picks = torch.zeros(K * 16, dtype=torch.uint8, device=dev)
+            detail = torch.zeros((K, stride), dtype=torch.uint8, device=dev)
+            kept_cost = torch.full((K,), math.nan, dtype=torch.float64, device=dev)
+            kept_usable = torch.zeros(K, dtype=torch.uint8, device=dev)
+            if kept is not None:
+                rec = self.records_device()[16 * kept:16 * (kept + 1)]
+                det = seg.detail_device(kept, kept + 1, self.records[kept:kept + 1], dev)
+            s = torch.cuda.current_stream(dev)
+            found = np.zeros(K, dtype=bool)
+            for first in range(0, K, chunk):
+                n = min(chunk, K - first)
+                probs = scenarios.stage(lib, p, first, n, s)
+                for k, pr in enumerate(probs):
+                    if pr is None:
+                        continue
+                    native.check(lib.metis_het_search(
+                        C.byref(pr), C.byref(sp), C.byref(shard), None, C.c_int64(0), None, C.c_int32(0), _ptr(sws),
+                        C.c_int64(sws.numel()), C.c_void_p(summaries.data_ptr() + size * (first + k)),
+                        C.c_void_p(s.cuda_stream)), 'metis_het_search')
+                if kept is not None:
+                    scenarios.eval_kept(lib, sp, first, n, rec, det, kept_cost, kept_usable, s)
+                s.synchronize()
+                for k in range(n):
+                    sm = native.MetisSearchSummary.from_buffer_copy(
+                        summaries.numpy()[size * (first + k):size * (first + k + 1)].tobytes())
+                    if sm.num_records == 0 or (sm.fatal_ordinal != _NO_FATAL and sm.fatal_code != 0):
+                        continue
+                    found[first + k] = True
+                    at = 16 * (first + k)
+                    picks_host.numpy()[at:at + 16] = np.frombuffer(bytes(sm.best), dtype=np.uint8)
+                    with torch.cuda.stream(s):
+                        picks[at:at + 16].copy_(picks_host[at:at + 16], non_blocking=True)
+                    native.check(lib.metis_het_detail(
+                        C.byref(probs[k]), C.byref(sp), _ptr(picks, at), C.c_int64(1), _ptr(detail, stride * (first + k)),
+                        C.c_int32(stride), _ptr(sws), C.c_int64(sws.numel()), C.c_void_p(s.cuda_stream)),
+                        'metis_het_detail')
+            out = [t.cpu().numpy() for t in (detail, kept_cost, kept_usable, scenarios.preset())]
+        detail, kept_cost, kept_usable, preset = out
+        raw = summaries.numpy().copy()
+        sums = [native.MetisSearchSummary.from_buffer_copy(raw[size * j:size * (j + 1)].tobytes()) for j in range(K)]
+        status = np.array([int(sm.fatal_code) if sm.fatal_ordinal != _NO_FATAL else 0 for sm in sums], dtype=np.int64)
+        status = np.where(preset != 0, preset, status)
+        found &= status == 0
+        count = np.array([int(sm.num_records) for sm in sums], dtype=np.int64)
+        best = np.zeros(K, dtype=native.RECORD_DTYPE)
+        best.view(np.uint8).reshape(K, 16)[:] = picks_host.numpy().reshape(K, 16)
+        winners = Candidates(best[found], detail[found], seg.space, self.node_sequences, rows_dev=seg._rows_dev)
+        return ScenarioSearch(self, kept, status, np.where(status == 0, count, 0), best, found, winners, kept_cost,
+                              kept_usable.astype(bool), within,
+                              {'search_s': time.perf_counter() - t0, 'chunks': -(-K // chunk), 'chunk': chunk})
 
     def records_device(self) -> torch.Tensor:
         """The records (estimate_costs order) on the device, uploaded on first use: what the replays and the group
@@ -1547,6 +1614,205 @@ class ProfileNoise:
                 raise ValueError(f'k must be >= 0, not {k}')
             pos = pos[:int(k)]
         return self.candidates.tuples(pos)
+
+
+# ---------------------------------------------------------------------------------------------
+# search what-if: a fresh search under each scenario profile (Candidates.search_scenarios)
+# ---------------------------------------------------------------------------------------------
+_SCENARIO_BUDGET_BYTES = 1 << 30         # device memory of one chunk of scenarios: their tables and staging
+
+
+def noise_spec(sigma, type_code: Sequence[int], seed: int, within: float) -> native.MetisNoiseSpec:
+    """The MetisNoiseSpec of a noise what-if: ``sigma`` [3, METIS_MAX_TYPES] and ``type_code`` per device type of the
+    searched problem, the seed and near_factor = 1.0 + ``within`` (first and count are set per chunk)."""
+    spec = native.MetisNoiseSpec()
+    for f in range(3):
+        for t in range(native.METIS_MAX_TYPES):
+            spec.sigma[f][t] = float(sigma[f][t])
+    for t, code in enumerate(type_code):
+        spec.type_code[t] = int(code)
+    spec.seed = int(seed)
+    spec.near_factor = 1.0 + float(within)
+    return spec
+
+
+def one_search_segment(candidates) -> 'SearchSegment':
+    """The one segment of a result searched at once; NotImplementedError naming the window count otherwise."""
+    segs = candidates.segments
+    if len(segs) != 1 or not isinstance(segs[0], SearchSegment):
+        raise NotImplementedError(f'a search what-if of a result searched in {len(segs)} windows: only results '
+                                  f'searched at once are supported')
+    return segs[0]
+
+
+class NoiseScenarios:
+    """Samples first .. first + count - 1 of noisy_profile, drawn on the device with their norm_lc
+    (metis_het_search_noise_*); the kept candidate is evaluated by metis_het_profile_noise_eval."""
+
+    def __init__(self, spec: native.MetisNoiseSpec, count: int, norm_row: Optional[np.ndarray], norm_code: int,
+                 norm_sigma: float):
+        self.spec, self.count = spec, count
+        self.norm = native.MetisNormSource(None, 0, norm_code, norm_sigma)
+        self._norm_row = norm_row
+        self._row = self._zero = self._ws = None
+
+    def reserve(self, lib, p, device) -> int:
+        """Allocates the device buffers of the call: the norm row, the zero-total flags and the draw workspace of one
+        chunk, sized under _SCENARIO_BUDGET_BYTES.  Returns the samples of a chunk."""
+        one = int(lib.metis_het_search_noise_workspace_bytes(C.byref(p), 1))
+        native.check(min(one, 0), 'metis_het_search_noise_workspace_bytes')
+        per = int(lib.metis_het_search_noise_workspace_bytes(C.byref(p), 2)) - one
+        n = int(max(1, min(self.count, (_SCENARIO_BUDGET_BYTES - one + per) // per)))
+        if self._norm_row is not None:
+            self._row = upload(np.ascontiguousarray(self._norm_row, dtype=np.float64), device)
+        self._zero = torch.zeros(self.count, dtype=torch.uint8, device=device)
+        self._ws = torch.empty(int(lib.metis_het_search_noise_workspace_bytes(C.byref(p), n)), dtype=torch.uint8,
+                               device=device)
+        return n
+
+    def search_bytes(self, lib, p, slots: int, max_stage: int) -> int:
+        need = int(lib.metis_het_workspace_bytes(C.byref(p), slots, max_stage))     # a sample's layout is the base's
+        native.check(min(need, 0), 'metis_het_workspace_bytes')
+        return need
+
+    def stage(self, lib, p, first: int, n: int, stream) -> List[native.MetisProblem]:
+        if self._row is None:                       # sigma 0 for the norm entry: the row is not read
+            self.norm.row, self.norm.len = p.norm_lc, p.norm_len
+        else:
+            self.norm.row, self.norm.len = self._row.data_ptr(), self._row.numel() // 8
+        self.spec.first, self.spec.count = first, n
+        native.check(lib.metis_het_search_noise_draw(C.byref(p), C.byref(self.spec), C.byref(self.norm), _ptr(self._ws),
+                                                     C.c_int64(self._ws.numel()), _ptr(self._zero, first),
+                                                     C.c_void_p(stream.cuda_stream)), 'metis_het_search_noise_draw')
+        out = []
+        for k in range(n):
+            pr = native.MetisProblem()
+            native.check(lib.metis_het_search_noise_problem(C.byref(p), C.byref(self.spec), C.c_int32(k),
+                                                            _ptr(self._ws), C.byref(pr)), 'metis_het_search_noise_problem')
+            out.append(pr)
+        return out
+
+    def eval_kept(self, lib, sp, first: int, n: int, rec, det, cost, usable, stream) -> None:
+        native.check(lib.metis_het_profile_noise_eval(
+            C.byref(sp), C.byref(self.spec), _ptr(self._ws), _ptr(rec), C.c_int64(1), _ptr(det),
+            C.c_int32(det.shape[1]), _ptr(cost, 8 * first), _ptr(usable, first), C.c_int64(1),
+            C.c_void_p(stream.cuda_stream)), 'metis_het_profile_noise_eval')
+
+    def preset(self) -> torch.Tensor:
+        """METIS_FATAL_ZERODIV where a sample's noisy norm total is 0, else 0."""
+        return self._zero.to(torch.int64) * native.FATAL_ZERODIV
+
+
+class ProfileScenarios:
+    """Caller-given profiles, each flattened with its own norm_lc (``problems``); ``zerodiv[j]``: profile j's norm
+    total is 0, so it is flattened with the searched norm_lc (as recost_profiles does) and not searched.  The kept
+    candidate is evaluated by metis_het_profile_recost."""
+
+    def __init__(self, problems: Sequence[flatten.FlatProblem], zerodiv: Sequence[bool]):
+        self.problems, self.count, self.device = list(problems), len(problems), None
+        self.zerodiv = np.asarray(zerodiv, dtype=bool)
+        self._bound = []
+
+    def reserve(self, lib, p, device) -> int:
+        """The scenarios of one chunk under _SCENARIO_BUDGET_BYTES (their tables are bound per chunk by stage)."""
+        self.device = device
+        per = max(int(lib.metis_het_workspace_bytes(C.byref(pr.as_struct(lambda n: 0)), 0, 1)) +
+                  sum(a.nbytes for a in pr.arrays.values()) for pr in self.problems)
+        return int(max(1, min(self.count, _SCENARIO_BUDGET_BYTES // max(2 * per, 1))))
+
+    def search_bytes(self, lib, p, slots: int, max_stage: int) -> int:
+        need = [int(lib.metis_het_workspace_bytes(C.byref(pr.as_struct(lambda n: 0)), slots, max_stage))
+                for pr in self.problems]
+        native.check(min(min(need), 0), 'metis_het_workspace_bytes')
+        return max(need)
+
+    def stage(self, lib, p, first: int, n: int, stream) -> List[native.MetisProblem]:
+        with torch.cuda.stream(stream):
+            self._bound = [bind_problem(pr, self.device, workspace=False) for pr in self.problems[first:first + n]]
+        return [b[1] if not self.zerodiv[first + k] else None for k, b in enumerate(self._bound)]
+
+    def eval_kept(self, lib, sp, first: int, n: int, rec, det, cost, usable, stream) -> None:
+        scen = (native.MetisProblem * n)(*[b[1] for b in self._bound])
+        need = int(lib.metis_het_profile_recost_workspace_bytes(C.c_void_p(C.addressof(scen)), C.c_int32(n)))
+        native.check(min(need, 0), 'metis_het_profile_recost_workspace_bytes')
+        with torch.cuda.stream(stream):
+            ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            head = torch.empty(n, dtype=torch.float64, device=self.device)
+            status = torch.empty(n, dtype=torch.uint8, device=self.device)
+            native.check(lib.metis_het_profile_recost(
+                C.byref(sp), C.c_void_p(C.addressof(scen)), C.c_int32(n), _ptr(rec), C.c_int64(1), _ptr(det),
+                C.c_int32(det.shape[1]), _ptr(cost, 8 * first), _ptr(head), _ptr(status), _ptr(ws),
+                C.c_int64(ws.numel()), C.c_void_p(stream.cuda_stream)), 'metis_het_profile_recost')
+            usable[first:first + n] = ((status == 0) & (head >= 0)).to(torch.uint8)
+
+    def preset(self) -> torch.Tensor:
+        return torch.from_numpy(self.zerodiv.astype(np.int64) * native.FATAL_ZERODIV)
+
+
+class ScenarioSearch:
+    """A fresh search under each of K scenario profiles P_j, next to the searched winner held fixed
+    (HetSearchResult.search_noise / search_profiles).  S_j is what api.cost_het_cluster returns under P_j (the searched
+    args, cluster, node sequences and corrections, the cost estimator and the layer balancer built from P_j, so its
+    norm_lc too); R the searched result.  Arrays of length K:
+
+      status           0, or the METIS_FATAL_* code with which cost_het_cluster under P_j raises (raise_fatal's
+                       mapping; a norm_lc total of 0 is METIS_FATAL_ZERODIV)
+      num_candidates   len(S_j), 0 when status != 0
+      best_cost        S_j.best()'s cost, bit for bit (NaN when S_j has no best)
+      kept_cost        R.best(), its device groups, strategies and partition fixed, under P_j: recost_profiles([P_j])'s
+      kept_usable      cost and usable flag (status 0 and headroom >= 0); NaN / False when R is empty
+      loss             kept_cost - best_cost when the kept plan is usable (not clamped: the balancer is not
+                       cost-optimal, so it can be negative), +inf when it is not, NaN when S_j has no best
+      near             kept usable and kept_cost <= best_cost * (1.0 + within)
+      same             winner(j)[:6] == R.best()[:6];  same_plan: the same ordinal (node sequence, device groups, batches)
+
+    ``winner(j)`` is S_j.best(), a 7-tuple, or None; ``winners()`` the distinct winners."""
+
+    def __init__(self, candidates, kept: Optional[int], status, num_candidates, best, found, winners, kept_cost,
+                 kept_usable, within: float, timings):
+        K = len(status)
+        self.status = status                            # int64 [K]
+        self.num_candidates = num_candidates            # int64 [K]
+        self._best = best                               # MetisRecord per scenario (valid where found)
+        self._found = found                             # bool [K]: S_j has a best
+        self._at = np.cumsum(found) - 1                 # scenario -> row of ``winners``
+        self._winners = winners
+        self.best_cost = np.where(found, best['cost'], np.nan)
+        self.kept_cost = kept_cost                      # float64 [K]
+        self.kept_usable = kept_usable                  # bool [K]
+        self.kept = None if kept is None else candidates.tuples([kept])[0]
+        with np.errstate(invalid='ignore'):
+            self.loss = np.where(~found, np.nan, np.where(kept_usable, kept_cost - self.best_cost, np.inf))
+            t = 1.0 + within
+            self.near = kept_usable & found & (kept_cost <= self.best_cost * t)
+        tuples = self._winners.tuples(np.arange(len(self._winners))) if len(self._winners) else []
+        self._tuples = [tuples[self._at[j]] if found[j] else None for j in range(K)]
+        kept_ordinal = -1 if kept is None else int(candidates.records['ordinal'][kept])
+        self.same = np.array([w is not None and self.kept is not None and w[:6] == self.kept[:6]
+                              for w in self._tuples], dtype=bool)
+        self.same_plan = found & (best['ordinal'].astype(np.int64) == kept_ordinal)
+        self.timings = timings
+
+    def __len__(self) -> int:
+        return len(self.status)
+
+    def winner(self, j) -> Optional[Tuple]:
+        """S_j.best(): the reference's 7-tuple, or None when S_j has no candidate or its search raises."""
+        return self._tuples[int(j)]
+
+    def winners(self) -> List[Tuple[Tuple, int, int]]:
+        """The distinct winners, (7-tuple of the first sample that picked it, count, that first sample), keyed by
+        ordinal, strategies, partition and num_repartition, by count descending, then first sample."""
+        seen: Dict[Tuple, List[int]] = {}
+        for j, t in enumerate(self._tuples):
+            if t is None:
+                continue
+            key = (int(self._best['ordinal'][j]), tuple(t[2]), tuple(t[4]), t[5])
+            if key in seen:
+                seen[key][1] += 1
+            else:
+                seen[key] = [j, 1]
+        return [(self._tuples[j], c, j) for j, c in sorted(seen.values(), key=lambda v: (-v[1], v[0]))]
 
 
 def materialize(records: np.ndarray, detail: np.ndarray, space: flatten.FlatPlanSpace,
